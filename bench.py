@@ -2,10 +2,10 @@
 """
 bench.py -- raw-signal samples/sec basecalled (forward + decode) on synthetic chunks.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload all|hac|sup]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload all|hac|sup] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-Headline workload (BASELINE.json configs[1], the one the metric is quoted on): hac-shaped LSTM-CRF (H=384, 5-mer scores,
+Headline workload (the one the metric is quoted on): hac-shaped LSTM-CRF (H=384, 5-mer scores,
 seeded random weights -- the real checkpoint needs the network), batch 512 chunks per GPU, 10 000-sample chunks trimmed
 to a stride multiple (9996) exactly as `_load_model(use_koi=True)` does (bonito/util.py:288-291).  A step = one batch
 through conv stem -> strided conv GEMM -> 5 x (input GEMM + persistent LSTM) -> CRF linear + clamp -> CRF decode.
@@ -16,16 +16,20 @@ through conv stem -> strided conv GEMM -> 5 x (input GEMM + persistent LSTM) -> 
          the timed region
   roofline / stages: per-kernel CUDA-event durations recorded inside the timed region
 
-`configs` (workload "all", the default) adds the other BASELINE.json configurations to the same JSON line:
+`configs` (workload "all", the default) adds the other configurations to the same JSON line:
   config3_sup        sup-shaped transformer (18 layers, d_model 512, k = 5), batch 256/GPU, 9996-sample chunks
   config5_sup_sweep  the same at chunk lengths 3996 / 7992 / 12000 (multiples of 12, SURVEY.md H6), batch 256/GPU
   config1_fast_cpu   fast-shaped LSTM-CRF, batch 8 x 4000 samples, the reference's PyTorch-CPU path on the host cores
-(config 4 is this script under torchrun: the driver runs N = 1, 2, 4, 8.)
+(config 4 is this script under torchrun with N = 1, 2, 4, 8.)
 
 Multi-GPU: chunks shard by batch (one process per GPU, weights broadcast once over NCCL, no steady-state collective)
 => weak scaling.
 --impl reference: the reference's PyTorch-CPU execution of the headline path (oracle/cpu_reference.py) on all host cores,
 a bounded sample of the workload per step.
+Every timed region runs exactly --steps steps after --warmup untimed ones.
+--dump-outputs DIR: after the timed steps of the headline workload (hac, or sup under --workload sup), the arrays its last
+step returned -- moves / sequence / qstring and the scores of a fixed, seeded sample of chunks -- as float32 DIR/<name>.npy
+(at most 64 MB in all); the inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -35,7 +39,7 @@ import sys
 import threading
 import time
 
-# The engine drives one CUDA stream per tile (11 + 11 at batch 512).  With the default of 8 hardware work queues, streams
+# The engine can drive one CUDA stream per tile (8 + 8 at batch 512).  With the default of 8 hardware work queues, streams
 # that share a queue serialise behind each other's not-yet-dispatched cluster launches; set before the CUDA context exists.
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
@@ -55,13 +59,40 @@ def log(msg):
     print(f"[bench {time.strftime('%H:%M:%S')}] {msg}", file=sys.stderr, flush=True)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, scores, decoded):
+    """What the last timed step returned, as float32 .npy files: the decoder's per-chunk outputs (moves, sequence, qstring)
+    and the scores, each for a fixed, seeded sample of chunks sized so that everything stays within DUMP_BYTES whatever the
+    batch (all scores of a batch are gigabytes); the sampled chunk indices go to chunks.npy."""
+    import numpy as np
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    n, t, c = scores.shape
+    rng = np.random.default_rng(0)
+    # at most 3/4 of the budget for scores, the rest for the three [chunks, T] decoder arrays
+    n_scores = max(1, min(n, 6, (DUMP_BYTES * 3 // 4) // (t * c * 4)))
+    n_dec = max(1, min(n, (DUMP_BYTES // 4) // (3 * t * 4)))
+    rows = np.sort(rng.choice(n, size=n_dec, replace=False))
+    srows = rows[np.sort(rng.choice(n_dec, size=min(n_dec, n_scores), replace=False))]
+    np.save(os.path.join(out_dir, "chunks.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "scores_chunks.npy"), srows.astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), scores[torch.as_tensor(srows, device=scores.device)].float().cpu().numpy())
+    for name, arr in zip(("moves", "sequence", "qstring"), decoded):
+        arr = torch.as_tensor(arr)
+        np.save(os.path.join(out_dir, f"{name}.npy"), arr[torch.as_tensor(rows, device=arr.device)].float().cpu().numpy())
+    log(f"outputs of the last timed step written to {out_dir}")
+
+
 def load_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
             p = json.load(fh)
         return dict(hbm=p["hbm_gbs"], tflops=p["bf16_tflops_sustained"], tflops_burst=p["bf16_tflops"], source="measured")
     except Exception:
-        return dict(hbm=6650.0, tflops=1400.0, tflops_burst=1590.0, source="fallback")
+        # NVIDIA's H100 SXM data sheet (dense fp16 / bf16, 700 W card): not measured here
+        return dict(hbm=3350.0, tflops=989.0, tflops_burst=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -263,13 +294,19 @@ def bench_hac(ctx, peaks, sampler):
     T = plan.frames(L)
     qs = model.config["qscore"]
 
+    last = {}
+
     def step(events, slot):
         scores = plan.forward(x_dev, events=events, slot=slot)
-        return _decoder(scores, spec["state_len"], blank_score=plan.blank_score, qscale=qs["scale"], qbias=qs["bias"],
-                        events=events, slot=slot)
+        decoded = _decoder(scores, spec["state_len"], blank_score=plan.blank_score, qscale=qs["scale"], qbias=qs["bias"],
+                           events=events, slot=slot)
+        last["scores"], last["decoded"] = scores, decoded
+        return decoded
 
     slots = N_SLOTS if plan.supports_slots else 1
-    elapsed_ms, events, enqueue_ms = time_resident(ctx, step, args.steps, max(args.warmup, 3), sampler, slots=slots)
+    elapsed_ms, events, enqueue_ms = time_resident(ctx, step, args.steps, args.warmup, sampler, slots=slots)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["scores"], last["decoded"])
     log(f"hac resident: {elapsed_ms / args.steps:.2f} ms/step ({slots} batches in flight)")
     e2e_ms = time_e2e(ctx, model, host_batch, args.steps, qs)
     for _ in range(2):
@@ -292,7 +329,7 @@ def bench_hac(ctx, peaks, sampler):
     tile_chunks = plan.tile if tile_mode else plan.TILE
     cluster = plan.tile_cs if tile_mode else 8
     n_tiles = -(-N // tile_chunks)
-    flops_step = {  # algorithmic FLOPs per step, all launches of the kernel (DESIGN.md section 4)
+    flops_step = {  # algorithmic FLOPs per step, all launches of the kernel
         "lstm_rec": spec["n_lstm"] * 2.0 * N * T * 4 * H * H,
         "lstm_in_gemm": spec["n_lstm"] * 2.0 * N * T * 4 * H * H,
         "conv_gemm": 2.0 * N * T * H * plan.k3 * plan.c2,
@@ -307,15 +344,9 @@ def bench_hac(ctx, peaks, sampler):
     peak_share = peaks["tflops"] * launch_sms / sms
     chip_ach = flops_step[dominant] / (step_ms * 1e-3) / 1e12
     traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as fh:
-            rec = json.load(fh)["lstm_rec_tile" if tile_mode else "lstm_rec"]
-            traffic = rec["bytes"] if N == BATCH and launches[dominant] == rec.get("launches_per_step", launches[dominant]) else None
-    except Exception:
-        pass
     chunks_per_launch = N * spec["n_lstm"] / launches[dominant]
-    roof = {"kernel": ("lstm_rec_tc6_kernel (persistent tcgen05 LSTM layer, one 6-CTA cluster per 48-chunk tile)" if tile_mode else
-                       "lstm_rec_tc_kernel (persistent tcgen05 LSTM layer, one 8-CTA cluster per 32-chunk tile)"),
+    roof = {"kernel": ("lstm_rec_tile_kernel (persistent wgmma LSTM layer, one 8-CTA cluster per 64-chunk tile)" if tile_mode else
+                       "lstm_rec_kernel (persistent mma.sync LSTM layer, one 8-CTA cluster per 32-chunk tile)"),
             "bound": "tensor", "achieved": ach, "peak": peak_share, "unit": "TFLOP/s", "frac": ach / peak_share,
             "traffic": traffic, "traffic_algorithmic": 2.0 * T * chunks_per_launch * 5 * H,
             "peak_source": f"{peaks['source']} sustained bf16 GEMM {peaks['tflops']} TFLOP/s x {launch_sms}/{sms} SMs "
@@ -327,11 +358,11 @@ def bench_hac(ctx, peaks, sampler):
     total_flops = sum(flops_step.values())
     line = {
         "metric": METRIC, "value": world * N * L * args.steps / (elapsed_ms * 1e-3), "unit": "samples/s",
-        "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": step_ms,
+        "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": step_ms,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": f"hac-shaped LSTM-CRF (H={H}, {spec['n_lstm']} LSTM, {plan.n_scores} scores/frame), "
                                f"batch {N}/GPU, {CHUNK}->{L}-sample chunks ({T} frames), forward+decode",
-                   "weights": "seeded synthetic (bonito_b200/synth.py)", "l2": "per-step tensors (0.16-2.6 GB) exceed the 126 MB L2",
+                   "weights": "seeded synthetic (bonito_b200/synth.py)", "l2": "per-step tensors (0.16-2.6 GB) exceed the 50 MB L2",
                    "parallelism": f"chunk-sharded replicas x{world}",
                    "batches_in_flight": slots},
         "e2e": {"value": world * N * L * args.steps / (e2e_ms * 1e-3), "unit": "samples/s",
@@ -365,8 +396,8 @@ def bench_hac_quantized(ctx):
         scores = plan.forward(x_dev, events=None, slot=slot)
         return _decoder(scores, spec["state_len"], blank_score=plan.blank_score, qscale=qs["scale"], qbias=qs["bias"], slot=slot)
 
-    steps = min(args.steps, 10)
-    elapsed_ms, _, _ = time_resident(ctx, step, steps, 3, None, slots=N_SLOTS if plan.supports_slots else 1)
+    steps = args.steps
+    elapsed_ms, _, _ = time_resident(ctx, step, steps, args.warmup, None, slots=N_SLOTS if plan.supports_slots else 1)
     (elapsed_ms,) = ctx.max_over_ranks([elapsed_ms])
     del model, plan
     torch.cuda.empty_cache()
@@ -390,7 +421,7 @@ def sup_flops(spec, plan, N, L):
             "crf_gemm": 2.0 * 2 * M * plan.n_scores * d}, Tq
 
 
-def bench_sup(ctx, peaks, model, spec, L, steps, warmup, with_e2e=True):
+def bench_sup(ctx, peaks, model, spec, L, steps, warmup, with_e2e=True, dump=None):
     """One sup configuration: batch 256 x L samples per GPU; returns the block that goes under `configs`."""
     from bonito_b200 import synth
     from bonito_b200.decode import _decoder
@@ -401,14 +432,20 @@ def bench_sup(ctx, peaks, model, spec, L, steps, warmup, with_e2e=True):
     plan = model.native_plan(device)
     qs = model.config["qscore"]
 
+    last = {}
+
     def step(events, slot):
         scores = plan.forward(x_dev, events=events, slot=slot)
-        return _decoder(scores, spec["state_len"], blank_score=plan.blank_score, qscale=qs["scale"], qbias=qs["bias"],
-                        events=events, slot=slot)
+        decoded = _decoder(scores, spec["state_len"], blank_score=plan.blank_score, qscale=qs["scale"], qbias=qs["bias"],
+                           events=events, slot=slot)
+        last["scores"], last["decoded"] = scores, decoded
+        return decoded
 
     # one batch at a time: the sup step is one long chain of chip-filling GEMMs, a second batch in flight buys nothing
     # (54.5 vs 56.2 ms measured) and would blur the per-kernel event times
     elapsed_ms, events, enqueue_ms = time_resident(ctx, step, steps, warmup, slots=1)
+    if dump and rank == 0:
+        dump_outputs(dump, last["scores"], last["decoded"])
     e2e_ms = time_e2e(ctx, model, host_batch, steps, qs) if with_e2e else 0.0
     elapsed_ms, e2e_ms = ctx.max_over_ranks([elapsed_ms, e2e_ms])
     log(f"sup L={L}: resident {elapsed_ms / steps:.2f} ms/step" + (f", e2e {e2e_ms / steps:.2f}" if with_e2e else ""))
@@ -495,7 +532,7 @@ def cpu_baseline(spec, weights, chunksize):
 
 
 def cpu_config1():
-    """BASELINE config 1: fast-shaped LSTM-CRF, batch 8 x 4000 samples, PyTorch-CPU, best of a few thread counts."""
+    """Config 1: fast-shaped LSTM-CRF, batch 8 x 4000 samples, PyTorch-CPU, best of a few thread counts."""
     from oracle import synth
     from oracle.cpu_reference import CpuReferenceModel
     spec = synth.model_spec("fast")
@@ -539,7 +576,7 @@ def run_reference(args, rank, world):
     _, threads, n_chunks, _, _, tried, x = _cpu_thread_sweep(ref, chunksize, "reference arm probe")
     torch.set_num_threads(threads)
     os.environ["OMP_NUM_THREADS"] = str(threads)
-    for _ in range(max(args.warmup, 1)):
+    for _ in range(args.warmup):
         ref.forward(x[:2])
     t0 = time.perf_counter()
     for _ in range(args.steps):
@@ -570,9 +607,11 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--batch", type=int, default=BATCH)
     ap.add_argument("--workload", default="all", choices=["all", "hac", "sup"],
-                    help="all: hac headline line + the other BASELINE configurations under `configs`; hac: headline only; "
+                    help="all: hac headline line + the other configurations under `configs`; hac: headline only; "
                          "sup: config 3 as the headline of the line")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the hac timed path computed in its last step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", 0))
@@ -614,18 +653,19 @@ def main():
         if args.workload in ("all", "sup"):
             model, spec = build_sup(device, rank, world)
             log("sup model built")
-            sup_steps, sup_warm = min(args.steps, 10), 3
+            sup_steps, sup_warm = args.steps, args.warmup
             if args.workload == "sup":
                 sampler = ClockSampler(local_rank)
                 if rank == 0:
                     sampler.start()
                     time.sleep(0.3)
                     sampler.mark_begin()
-            c3 = bench_sup(ctx, peaks, model, spec, 9996, sup_steps, sup_warm)
+            c3 = bench_sup(ctx, peaks, model, spec, 9996, sup_steps, sup_warm,
+                           dump=args.dump_outputs if args.workload == "sup" else None)
             if args.workload == "sup" and rank == 0:
                 sampler.mark_end()
                 clocks = sampler.stop()
-            sweep = [bench_sup(ctx, peaks, model, spec, L, max(3, sup_steps // 2), 3, with_e2e=False) for L in SUP_SWEEP]
+            sweep = [bench_sup(ctx, peaks, model, spec, L, sup_steps, sup_warm, with_e2e=False) for L in SUP_SWEEP]
             if rank == 0:
                 configs["config3_sup"] = c3
                 configs["config5_sup_sweep"] = [{k: b[k] for k in ("workload", "value", "unit", "n_gpus", "ms_per_step",
@@ -641,7 +681,7 @@ def main():
                     "ms_per_step": c3["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                     "dtype": "f16", "data": "synthetic",
                     "config": {"workload": c3["workload"], "weights": "seeded synthetic (bonito_b200/synth.py)",
-                               "l2": "per-step tensors (0.2-3.5 GB) exceed the 126 MB L2",
+                               "l2": "per-step tensors (0.2-3.5 GB) exceed the 50 MB L2",
                                "parallelism": f"chunk-sharded replicas x{world}"},
                     "e2e": c3["e2e"], "gpu_launches": c3["gpu_launches"], "roofline": c3["roofline"],
                     "stage_ms_per_step": c3["stage_ms_per_step"], "stage_tflops": c3["stage_tflops"],

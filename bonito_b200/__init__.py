@@ -1,8 +1,8 @@
 """
-bonito_b200: B200-native drop-in for the chunked forward + decode path of nanoporetech/bonito.
+bonito_b200: H100-native drop-in for the chunked forward + decode path of nanoporetech/bonito.
 
 Mirrors the reference's plugin surface for that path (`bonito.nn` registry, `bonito.util`
-loader / chunking helpers, `bonito.crf.Model` + `basecall`) over hand-written sm_100a kernels
+loader / chunking helpers, `bonito.crf.Model` + `basecall`) over hand-written sm_90a kernels
 reached through the C ABI in include/bonito_b200.h.
 """
 

@@ -1,4 +1,4 @@
-"""`python -m bonito_b200 <subcommand>`: argparse sub-command dispatch as in `/root/reference/bonito/__init__.py:14-32`."""
+"""`python -m bonito_b200 <subcommand>`: argparse sub-command dispatch as in `bonito/__init__.py:14-32`."""
 from argparse import ArgumentParser, ArgumentDefaultsHelpFormatter
 
 from bonito_b200 import __version__

@@ -1,6 +1,6 @@
 """
 `bonito_b200 basecaller <model_directory> <reads_directory>` -- the flag surface of the reference's
-`bonito basecaller` (`/root/reference/bonito/cli/basecaller.py:168-199`) over the B200 engine.
+`bonito basecaller` (`bonito/cli/basecaller.py:168-199`) over the native engine.
 Alignment (`--reference`, needs mappy) and CTC training-data export (`--save-ctc`) are outside the hot path and
 exit with an explanation; output is unaligned FASTQ, or unaligned SAM text with the `mv:B:c` move table when stdout is
 redirected to a `.sam` file (the reference's `biofmt` rule, bonito/io.py:35-54).
@@ -53,10 +53,10 @@ def main(args):
         sys.stderr.write(f"> error: failed to load {args.model_directory}\n")
         exit(1)
     try:
-        # build the native plan now: a layer stack without a B200 kernel is reported here, not from the writer thread
+        # build the native plan now: a layer stack without a native kernel is reported here, not from the writer thread
         model.native_plan()
     except NotImplementedError as err:          # engine.UnsupportedModel
-        sys.stderr.write(f"> error: no native B200 path for this model (there is no eager fallback): {err}\n")
+        sys.stderr.write(f"> error: no native path for this model (there is no eager fallback): {err}\n")
         exit(1)
     if args.verbose:
         sys.stderr.write(f"> model basecaller params: {model.config['basecaller']}\n")

@@ -1,8 +1,8 @@
 """
 Chunked basecalling: chunk -> batch -> forward -> decode -> stitch -> format.
 
-Same generator graph and result contract as `/root/reference/bonito/crf/basecall.py:13-82`; the
-forward pass and the decoder are the sm_100a kernels behind `model(...)` and
+Same generator graph and result contract as `bonito/crf/basecall.py:13-82`; the
+forward pass and the decoder are the sm_90a kernels behind `model(...)` and
 `bonito_b200.decode.beam_search`.  Host staging differs from the reference in one respect that does not
 change results: the fp16 cast happens into a pinned buffer and the copy is asynchronous.
 """

@@ -1,8 +1,8 @@
 """
 CTC-CRF model package (`Model`, `basecall` are what `load_symbol` looks up:
-`/root/reference/bonito/util.py:223-234`, `/root/reference/bonito/cli/basecaller.py:71`).
+`bonito/util.py:223-234`, `bonito/cli/basecaller.py:71`).
 
-Inference-only mirror of `/root/reference/bonito/crf/model.py`: the state graph (`CTC_CRF`),
+Inference-only mirror of `bonito/crf/model.py`: the state graph (`CTC_CRF`),
 `SeqdistModel` and `Model` with the `use_koi` swap-in hook.  Training losses (koi.ctc) are out
 of scope (SURVEY.md section 2a row 12).
 """
@@ -113,7 +113,7 @@ class SeqdistModel(Module):
         """
         Plain module tree ([T, N, C+blanks], the reference's non-koi path) unless `use_koi` armed the
         native engine, in which case the result is [N, T, C] fp16 without blank column and any failure to
-        reach the sm_100a kernels raises (no CPU fallback).
+        reach the sm_90a kernels raises (no CPU fallback).
         """
         if self._native is None:
             if x.is_cuda:
@@ -158,14 +158,14 @@ class SeqdistModel(Module):
         return super().load_state_dict(*args, **kwargs)
 
     def use_koi(self, **kwargs):
-        """Arm the B200 engine (the hook `_load_model` calls: bonito/util.py:292-296)."""
+        """Arm the native engine (the hook `_load_model` calls: bonito/util.py:292-296)."""
         self._native = dict(kwargs)
         self._plan = None
 
     # -- decode ------------------------------------------------------------------------------------
     def decode_batch(self, x):
         """
-        x: scores.  Native layout [N, T, C] (no blanks) on CUDA -> list of N strings, via the sm_100a
+        x: scores.  Native layout [N, T, C] (no blanks) on CUDA -> list of N strings, via the sm_90a
         posterior-Viterbi kernel (same maths as the reference's decode_batch, bonito/crf/model.py:196-199).
         """
         from bonito_b200.decode import beam_search, to_str

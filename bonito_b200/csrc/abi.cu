@@ -19,22 +19,11 @@ int launch_rmsnorm_residual(const __half* a, const __half* x, const __half* w, f
 int launch_swiglu(const __half* h, __half* out, long long M, int F, cudaStream_t stream);
 int launch_attention(__half* qkv, const __half* cos_sin, __half* out, int N, int T, int NH, int head_dim, int wl,
                      int wr, cudaStream_t stream);
-bool lstm_rec_tc_supported(int hidden);
-int launch_lstm_rec_tc(const __half* gx, const __half* whh, __half* y, int T, int N, int hidden, int reverse,
-                       cudaStream_t stream);
-int launch_tmem_probe(float* out, cudaStream_t stream);
 int lstm_rec_tile_chunks(int hidden);
 int lstm_rec_tile_cluster(int hidden);
-int launch_lstm_rec_tc6(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
-                        int reverse, cudaStream_t stream);
+int launch_lstm_rec_tile(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
+                         int reverse, cudaStream_t stream);
 size_t lstm_rec_tile_workspace_bytes(int N);
-int copy_lstm_timeline6(long long* host_out, int max_steps);
-int copy_lstm_timeline(long long* host_out, int max_steps);
-int lstm_rec_tc_max_clusters();
-int debug_max_clusters(int cluster_size, int threads, int smem_bytes);
-int launch_exchange_bench(int mode, int steps, int delay, int clusters, unsigned char* staging, long long* out,
-                          cudaStream_t stream);
-int launch_mma_bench(int ts_mode, int n, int iters, int chains, int blocks, long long* out, cudaStream_t stream);
 size_t crf_decode_workspace_bytes(int N, int T, int state_len);
 int launch_crf_decode(const __half* scores, int N, int T, int state_len, float blank, float qscale, float qbias,
                       void* workspace, uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream);
@@ -45,8 +34,6 @@ int launch_crf_beam_search(const __half* scores, int N, int T, int state_len, fl
                            float qbias, void* workspace, uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream);
 
 int launch_lstm_crf_fwd(const b200_lstm_crf_plan* p, const __half* x, __half* scores, cudaStream_t stream);
-
-int copy_attention_timeline(long long* host_out, int max_tiles);
 
 int launch_quantize_i8(const __half* x, int8_t* out, long long n, float scale, cudaStream_t stream);
 int launch_gemm_i8(const int8_t* A, long long lda, const int8_t* B, const float* col_scale, __half* C, long long ldc, int M,
@@ -98,7 +85,8 @@ int b200_gemm_fwd_ex(const void* a, long long lda, const void* b, const void* bi
                  cb_width);
     if (act == B200_ACT_SWIGLU)
         B200_REQUIRE(n % 64 == 0 && !bias && impl != B200_GEMM_MMA_SYNC,
-                     "gemm: the fused SwiGLU epilogue needs n %% 64 == 0, no bias and the tcgen05 path (n=%d)", n);
+                     "gemm: the fused SwiGLU epilogue needs n %% 64 == 0, no bias and the wgmma path (n=%d)", n);
+    B200_REQUIRE(impl == B200_GEMM_AUTO || impl == B200_GEMM_TCGEN05 || impl == B200_GEMM_MMA_SYNC, "gemm: unknown impl %d", impl);
     if (m == 0) return 0;
     GemmEpilogue ep;
     ep.bias = (const __half*)bias;
@@ -121,7 +109,7 @@ int b200_gemm_fwd_ex(const void* a, long long lda, const void* b, const void* bi
         return launch_gemm_mma((const __half*)a, lda, (const __half*)b, (__half*)c, ldc, m, n, k, ep,
                                (cudaStream_t)stream);
     return launch_gemm_tc((const __half*)a, lda, (const __half*)b, (__half*)c, ldc, m, n, k, ep, max_ctas,
-                          (cudaStream_t)stream, impl == B200_GEMM_TCGEN05_PAIR);
+                          (cudaStream_t)stream);
 }
 
 int b200_conv_first_fwd(const void* x, int n, int l, int c, int k, const void* w, const void* bias, int act, void* out,
@@ -163,11 +151,6 @@ int b200_lstm_rec_fwd(const void* gx, const void* whh, void* y, int t, int n, in
     B200_REQUIRE(gx && whh && y, "lstm_rec: null pointer argument");
     B200_REQUIRE(t >= 0 && n >= 0, "lstm_rec: bad sizes t=%d n=%d", t, n);
     if (t == 0 || n == 0) return 0;
-    const char* env = getenv("B200_LSTM_IMPL");
-    const bool force_mma = env && strcmp(env, "mma") == 0;
-    if (!force_mma && lstm_rec_tc_supported(hidden))
-        return launch_lstm_rec_tc((const __half*)gx, (const __half*)whh, (__half*)y, t, n, hidden, reverse,
-                                  (cudaStream_t)stream);
     return launch_lstm_rec((const __half*)gx, (const __half*)whh, (__half*)y, t, n, hidden, reverse,
                            (cudaStream_t)stream);
 }
@@ -183,51 +166,8 @@ int b200_lstm_rec_tile_fwd(const void* gx, const void* whh, void* y, void* works
     B200_REQUIRE(gx && whh && y && workspace, "lstm_rec_tile: null pointer argument");
     B200_REQUIRE(t >= 0 && n >= 0, "lstm_rec_tile: bad sizes t=%d n=%d", t, n);
     if (t == 0 || n == 0) return 0;
-    return launch_lstm_rec_tc6((const __half*)gx, (const __half*)whh, (__half*)y, workspace, t, n, hidden, reverse,
+    return launch_lstm_rec_tile((const __half*)gx, (const __half*)whh, (__half*)y, workspace, t, n, hidden, reverse,
                                (cudaStream_t)stream);
-}
-
-int b200_debug_lstm_tile_timeline(long long* host_out, int max_steps) {
-    B200_REQUIRE(host_out != nullptr && max_steps > 0, "lstm_tile_timeline: bad arguments");
-    return copy_lstm_timeline6(host_out, max_steps);
-}
-
-int b200_debug_attention_timeline(long long* host_out, int max_tiles) {
-    B200_REQUIRE(host_out != nullptr && max_tiles > 0, "attention_timeline: bad arguments");
-    return copy_attention_timeline(host_out, max_tiles);
-}
-
-int b200_debug_gemm_profile(long long* host_out) {
-    B200_REQUIRE(host_out != nullptr, "gemm_profile: null pointer argument");
-    return copy_gemm_profile(host_out);
-}
-
-int b200_debug_tmem_probe(void* out, void* stream) {
-    B200_REQUIRE(out != nullptr, "tmem_probe: null pointer argument");
-    return launch_tmem_probe((float*)out, (cudaStream_t)stream);
-}
-
-int b200_debug_lstm_max_clusters(void) { return lstm_rec_tc_max_clusters(); }
-
-int b200_debug_exchange_bench(int mode, int steps, int delay, int clusters, void* staging, void* out, void* stream) {
-    B200_REQUIRE(staging && out && steps > 0 && clusters > 0 && clusters <= 22 && (mode == 0 || (mode >= 2 && mode <= 4)),
-                 "exchange_bench: bad arguments");
-    return launch_exchange_bench(mode, steps, delay, clusters, (unsigned char*)staging, (long long*)out, (cudaStream_t)stream);
-}
-
-int b200_debug_max_clusters(int cluster_size, int threads, int smem_bytes) {
-    return debug_max_clusters(cluster_size, threads, smem_bytes);
-}
-
-int b200_debug_lstm_timeline(long long* host_out, int max_steps) {
-    B200_REQUIRE(host_out != nullptr && max_steps > 0, "lstm_timeline: bad arguments");
-    return copy_lstm_timeline(host_out, max_steps);
-}
-
-int b200_debug_mma_bench(int ts_mode, int n, int iters, int chains, int blocks, void* out, void* stream) {
-    B200_REQUIRE(out != nullptr && n >= 16 && n <= 256 && n % 16 == 0 && iters > 0 && chains >= 1 && chains * n <= 448,
-                 "mma_bench: bad arguments");
-    return launch_mma_bench(ts_mode, n, iters, chains, blocks, (long long*)out, (cudaStream_t)stream);
 }
 
 size_t b200_crf_decode_workspace_bytes(int n, int t, int state_len) {

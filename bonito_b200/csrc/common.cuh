@@ -1,4 +1,4 @@
-// Shared device/host helpers for the bonito_b200 sm_100a kernels.
+// Shared device/host helpers for the bonito_b200 sm_90a kernels.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -58,6 +58,24 @@ __device__ __forceinline__ float tanh_f(float x) {
 }
 
 __device__ __forceinline__ float swish_f(float x) { return x * sigmoid_f(x); }
+
+// sigma(i), sigma(f), tanh(g), sigma(o) from four ex2 and ONE reciprocal (batch inversion); the exponent arguments are
+// clamped so the product of the four denominators stays finite (sigma(-20.8) = 9e-10: the clamp is invisible in fp16).
+__device__ __forceinline__ void gate_activations(float ai, float af, float ag, float ao, float& si, float& sf, float& tg,
+                                                 float& so) {
+    constexpr float L = 1.4426950408889634f, CLAMP = 30.0f;
+    const float di = 1.0f + ex2_approx(fminf(-L * ai, CLAMP));
+    const float df = 1.0f + ex2_approx(fminf(-L * af, CLAMP));
+    const float dg = 1.0f + ex2_approx(fminf(-2.0f * L * ag, CLAMP));
+    const float dO = 1.0f + ex2_approx(fminf(-L * ao, CLAMP));
+    const float pif = di * df, pgo = dg * dO;
+    const float r = rcp_approx(pif * pgo);
+    const float rif = r * pgo, rgo = r * pif;
+    si = rif * df;
+    sf = rif * di;
+    tg = fmaf(2.0f, rgo * dO, -1.0f);
+    so = rgo * dg;
+}
 
 // Apply an epilogue activation to a value that the reference would already have
 // rounded to fp16 (conv/linear output), then round again (elementwise op output).
@@ -142,11 +160,10 @@ struct GemmEpilogue {
 };
 
 // Host-side launchers (defined in the .cu files, used by abi.cu)
-int copy_gemm_profile(long long* host_out);
 int chunk_count(long long length, int chunksize, int overlap);
 int launch_chunk_signal(const void* signal, int is_f32, long long length, int chunksize, int overlap, __half* out,
                         long long row_stride, cudaStream_t stream);
 int launch_gemm_mma(const __half* A, long long lda, const __half* B, __half* C, long long ldc, int M, int N, int K,
                     const GemmEpilogue& ep, cudaStream_t stream);
 int launch_gemm_tc(const __half* A, long long lda, const __half* B, __half* C, long long ldc, int M, int N, int K,
-                   const GemmEpilogue& ep, int max_ctas, cudaStream_t stream, bool force_pair = false);
+                   const GemmEpilogue& ep, int max_ctas, cudaStream_t stream);

@@ -8,8 +8,8 @@
 int launch_conv_stem(const __half* x, int N, int L, int C1, int K1, const __half* w1, const __half* b1, int act1,
                      int C2, int K2, const __half* w2, const __half* b2, int act2, __half* out, int Lp, int padl,
                      cudaStream_t stream);
-int launch_lstm_rec_tc6(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
-                        int reverse, cudaStream_t stream);
+int launch_lstm_rec_tile(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
+                         int reverse, cudaStream_t stream);
 int lstm_rec_tile_chunks(int hidden);
 int lstm_rec_tile_cluster(int hidden);
 size_t lstm_rec_tile_workspace_bytes(int N);
@@ -44,7 +44,7 @@ int launch_lstm_crf_fwd(const b200_lstm_crf_plan* p, const __half* x, __half* sc
         ep.cb_width = CW; ep.cb_rows = TB;
         rc = launch_gemm_tc(cur, H, (const __half*)p->wih[i], gx, CW, nt * T * TB, 4 * H, H, ep, 0, stream);
         if (rc) return rc;
-        rc = launch_lstm_rec_tc6(gx, (const __half*)p->whh[i], nxt, p->hx, T, N, H, p->reverse[i], stream);
+        rc = launch_lstm_rec_tile(gx, (const __half*)p->whh[i], nxt, p->hx, T, N, H, p->reverse[i], stream);
         if (rc) return rc;
         __half* tmp = cur; cur = nxt; nxt = tmp;
     }

@@ -1,8 +1,8 @@
 // C[M,N] = epilogue(A[M,K] * B[N,K]^T) -- legacy tensor path (mma.sync m16n8k16).
 //
-// Bring-up / cross-check implementation: it is what the tcgen05 GEMM in gemm_tc.cu is
-// validated against on the device (tests/test_gpu_gemm.py) and is selectable at run time
-// with B200_GEMM_IMPL=mma.  Not the product path.
+// Cross-check implementation: the wgmma GEMM in gemm_wgmma.cu is validated against it on the
+// device (tests/test_gpu_kernels.py) and it is selectable at run time with B200_GEMM_IMPL=mma.
+// Not the product path.
 //
 // A rows may overlap (lda < K): conv3 of the LSTM-CRF encoder is run as a GEMM over the
 // channels-last, zero-padded output of the conv stem, where row t is the 19x16 window that

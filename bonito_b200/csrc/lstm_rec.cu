@@ -131,9 +131,17 @@ lstm_rec_kernel(const __half* __restrict__ gx, const __half* __restrict__ whh, _
                 float af = acc[0][j][2 + e] + __high2float(g01);
                 float ag = acc[1][j][e] + __low2float(g23);
                 float ao = acc[1][j][2 + e] + __high2float(g23);
-                float c = sigmoid_f(af) * c_state[j][e] + sigmoid_f(ai) * tanh_f(ag);
+                float c, h;
+                if constexpr (H == 384) {   // the cell math of the tile kernel: the two width-384 kernels agree bitwise
+                    float si, sf, tg, so;
+                    gate_activations(ai, af, ag, ao, si, sf, tg, so);
+                    c = fmaf(sf, c_state[j][e], si * tg);
+                    h = so * tanh_f(c);
+                } else {
+                    c = sigmoid_f(af) * c_state[j][e] + sigmoid_f(ai) * tanh_f(ag);
+                    h = sigmoid_f(ao) * tanh_f(c);
+                }
                 c_state[j][e] = c;
-                float h = sigmoid_f(ao) * tanh_f(c);
                 int b = nh * 16 + j * 8 + 2 * q + e;
                 stage[b * LDS + unit_local] = __float2half_rn(h);
             }

@@ -1,12 +1,11 @@
-// PTX wrappers shared by the tcgen05 kernels (sm_100a): mbarriers, TMA, UMMA descriptors, TMEM access,
-// cluster / distributed-shared-memory helpers.
+// PTX wrappers shared by the Hopper tensor-core kernels (sm_90a): mbarriers, bulk copies, cluster / distributed-shared-memory
+// helpers, wgmma descriptors and fences.
 #pragma once
 
 #include "common.cuh"
 
 // One lane of a converged warp (elect.sync): unlike `lane == 0`, the compiler then knows the guarded code runs in a
-// single thread and feeds UTCHMMA / UTMALDG from uniform registers directly instead of wrapping every instruction in
-// an R2UR + ELECT + BRA.U.ANY loop (~48 cycles per MMA issue).
+// single thread and can issue bulk copies from uniform registers.
 __device__ __forceinline__ bool elect_one_sync() {
     uint32_t pred;
     asm volatile(
@@ -97,145 +96,36 @@ __device__ __forceinline__ void bulk_copy_to_peer(uint32_t peer_dst, uint32_t lo
                  : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-// make generic-proxy writes (st.shared / st.shared::cluster) visible to the async proxy (UMMA / TMA reads)
+// make generic-proxy writes (st.shared / st.shared::cluster) visible to the async proxy (wgmma / bulk-copy reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;\n" ::: "memory"); }
 
-// ---- tcgen05 ------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_alloc(uint32_t slot_smem_addr, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(slot_smem_addr), "r"(ncols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-}
-__device__ __forceinline__ void tc_dealloc(uint32_t tmem_base, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(ncols));
-}
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void tc_mma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem, s32] (+)= A[smem, int8] * B[smem, int8]
-__device__ __forceinline__ void tc_mma_ss_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void tc_mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// instruction descriptor: D=f32, A=B=f16, both K-major; N at [17,23) (>>3), M at [24,29) (>>4)
-__device__ __forceinline__ constexpr uint32_t tc_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// K-major, 128-byte swizzled operand tile: rows of 64 fp16 (128 B), 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t tc_smem_desc_sw128(uint32_t smem_addr) {
+// ---- wgmma --------------------------------------------------------------------------------------
+// Operand tiles are K-major WITHOUT swizzle: core matrices of 8 rows x 16 bytes (128 contiguous bytes); `lbo` = byte
+// distance between core matrices adjacent along K, `sbo` = between adjacent 8-row groups along M / N.
+__device__ __forceinline__ uint64_t wg_desc_noswz(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
     uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address            bits [0,14)
-    d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset       bits [32,46)
-    d |= (uint64_t)1 << 46;                        // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                        // SWIZZLE_128B
-    return d;
+    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address        bits [0,14)
+    d |= (uint64_t)(lbo >> 4) << 16;               // leading byte offset  bits [16,30)
+    d |= (uint64_t)(sbo >> 4) << 32;               // stride byte offset   bits [32,46)
+    return d;                                      // layout type 0 (no swizzle) in bits [62,64)
 }
-// K-major operand tile WITHOUT swizzle: 8-row x 16-byte core matrices (128 contiguous bytes); `lbo` = byte distance
-// between core matrices adjacent along K, `sbo` = between adjacent 8-row groups.
-__device__ __forceinline__ uint64_t tc_smem_desc_noswz(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(lbo >> 4) << 16;
-    d |= (uint64_t)(sbo >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-// byte offset of (row, 16-byte chunk) inside a K-major SWIZZLE_128B tile whose rows are 128 B
-__device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
-    return (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma (the constraint matches the
+// register type, so no conversion moves land between the wgmma and its commit / wait)
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(int (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
-// 32 lanes x 32 columns (thread i <-> lane base+i)
-__device__ __forceinline__ void tc_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tc_st_32x32b_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31};\n" ::"r"(v[0]),
-        "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-        "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]),
-        "r"(v[29]), "r"(v[30]), "r"(v[31]), "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tc_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_32x32b_x1(uint32_t taddr, uint32_t& v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];\n" : "=r"(v) : "r"(taddr));
-}
-__device__ __forceinline__ void tc_st_32x32b_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15};\n" ::"r"(v[0]),
-        "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(taddr)
-        : "memory");
-}
-// 16 lanes x 4 groups of 256 bit: the mma accumulator-style fragment
-//   v[4j+0..1] = (row i/4,   cols 8j + 2(i%4) + {0,1});  v[4j+2..3] = (row i/4 + 8, same cols)
-__device__ __forceinline__ void tc_ld_16x256b_x4(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.16x256b.x4.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_16x256b_x1(uint32_t taddr, uint32_t (&v)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.16x256b.x1.b32 {%0,%1,%2,%3}, [%4];\n"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_16x256b_x2(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.16x256b.x2.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
+#include "wgmma_ops.cuh"

@@ -1,6 +1,6 @@
 // Kernels of the transformer (sup v5) path that are not GEMMs.  Reference semantics:
 //   conv_first      bonito/nn.py:221-241  Convolution(1 -> C, k, 'same') + Swish, written channels-last + zero halo so
-//                   that every following Convolution is a tcgen05 GEMM over overlapping rows (gemm_tc.cu)
+//                   that every following Convolution is a wgmma GEMM over overlapping rows (gemm_wgmma.cu)
 //   attention       bonito/transformer/model.py:42-79  rotary (flash_attn/layers/rotary.py, NeoX half rotation, fp16 cos/sin)
 //                   + flash_attn_qkvpacked_func(window_size=(wl, wr)), non-causal, softmax scale 1/sqrt(head_dim)
 //   rmsnorm         bonito/transformer/model.py:126-127  x = RMSNorm(sublayer(x), residual = alpha * x)
@@ -8,7 +8,7 @@
 //                   fp16 multiply in the reference because deepnorm_alpha is a half buffer)
 //   swiglu          flash_attn/ops/activations.py:107-111  float(gate) * float(y) / (1 + exp(-gate)), rounded once
 // First correct versions: attention runs on the legacy mma.sync path (it is ~6 % of the layer's FLOPs because of the
-// 256-wide window); the GEMMs, 94 % of the work, are the tcgen05 kernels.
+// 256-wide window); the GEMMs are the wgmma kernels.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -383,20 +383,19 @@ int launch_swiglu(const __half* h, __half* out, long long M, int F, cudaStream_t
     return 0;
 }
 
-bool attention_tc_supported(int head_dim, int wl, int wr);
-int launch_attention_tc(const __half* qkv, __half* out, int N, int T, int NH, int wl, int wr, cudaStream_t stream);
+int launch_attention_wgmma(const __half* qkv, __half* out, int N, int T, int NH, int wl, int wr, cudaStream_t stream);
 
 int launch_attention(__half* qkv, const __half* cos_sin, __half* out, int N, int T, int NH, int head_dim, int wl,
                      int wr, cudaStream_t stream) {
     B200_REQUIRE(head_dim == HD, "attention: head_dim %d is not supported (64)", head_dim);
     const long long tokens = (long long)N * T, work = tokens * 2 * NH * 4;
     rotary_kernel<<<(unsigned)((work + 255) / 256), 256, 0, stream>>>(qkv, cos_sin, tokens, T, NH);
-    // product path: tcgen05 kernel (attention_tc.cu) for windows of at most 128 keys each way (sup v5: 127 / 128);
-    // B200_ATTN_IMPL=mma keeps the mma.sync kernel below as an on-device cross-check, and it serves every other window
+    // product path: the wgmma kernel (attention_wgmma.cu); B200_ATTN_IMPL=mma runs the mma.sync kernel below (on-device
+    // cross-check)
     const char* impl = getenv("B200_ATTN_IMPL");
-    if (!(impl && impl[0] == 'm') && attention_tc_supported(head_dim, wl, wr)) {
+    if (!(impl && impl[0] == 'm')) {
         B200_CHECK_CUDA(cudaGetLastError());
-        return launch_attention_tc(qkv, out, N, T, NH, wl, wr, stream);
+        return launch_attention_wgmma(qkv, out, N, T, NH, wl, wr, stream);
     }
     if (wl < 0) wl = T;
     if (wr < 0) wr = T;

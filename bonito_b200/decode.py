@@ -1,10 +1,10 @@
 """
 Decoder op with the call contract of `koi.decode.beam_search` / `to_str`
-(`/root/reference/bonito/crf/basecall.py:7,36-40,50-54`).
+(`bonito/crf/basecall.py:7,36-40,50-54`).
 
 koi's beam search is a closed binary with no pinned outputs (SURVEY.md section 8c), so the default
 arithmetic here is the reference's in-repo decode definition (`SeqdistModel.decode_batch`,
-`/root/reference/bonito/crf/model.py:196-199`): exact forward-backward posteriors followed by a Viterbi
+`bonito/crf/model.py:196-199`): exact forward-backward posteriors followed by a Viterbi
 pass over the log-posteriors; `beam_width` and `beam_cut` are then unused (the search is exact).
 
 `decoder="beam"` (or `B200_DECODER=beam` in the environment) runs this repository's own beam search

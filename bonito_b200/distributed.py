@@ -1,6 +1,6 @@
 """
 Read-sharded multi-GPU execution (SURVEY.md section 8e): one process per GPU, chunks are independent from
-`chunk()` to `stitch()` (`/root/reference/bonito/crf/basecall.py:63-77`), so the only collective on the path is one
+`chunk()` to `stitch()` (`bonito/crf/basecall.py:63-77`), so the only collective on the path is one
 broadcast of the parameters at start-up.  The reference itself has no multi-device support (single `--device`,
 `bonito/cli/basecaller.py:177`).
 """

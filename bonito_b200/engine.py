@@ -2,7 +2,7 @@
 Plan builder + executor for the LSTM-CRF encoder (the `bonito.crf` fast / hac models; LSTM widths 96, 128, 256, 384).
 
 `compile_lstm_crf(encoder)` walks a `bonito_b200.nn` module tree of the shape the reference's
-configs describe (`/root/reference/bonito/models/configs/dna_r10.4.1@v4.3.toml`,
+configs describe (`bonito/models/configs/dna_r10.4.1@v4.3.toml`,
 `bonito/crf/model.py:150-162`):
 
     Convolution(1->C1,k5) , Convolution(C1->C2,k5) , Convolution(C2->H,kW,stride s)
@@ -10,20 +10,19 @@ configs describe (`/root/reference/bonito/models/configs/dna_r10.4.1@v4.3.toml`,
 
 (LinearCRFEncoder: a plain linear head followed by a Clamp layer, as in the v4+ configs, or the old-style head with
 activation = "tanh" and / or a scale and no Clamp; fixed blank_score) and packs the weights into the operand layouts of
-the sm_100a kernels (include/bonito_b200.h).  This is the native swap-in the reference performs in `Model.use_koi`
+the sm_90a kernels (include/bonito_b200.h).  This is the native swap-in the reference performs in `Model.use_koi`
 (`bonito/crf/model.py:240-246`, koi.lstm.update_graph); like koi it returns scores as `[N, T, C]` fp16 without the blank
 column.  Anything else raises `UnsupportedModel`.
 
-Width 384 (hac), the headline path (`forward_tiles`, DESIGN.md sections 3 and 4): activations tile-major
-`[tile][T][48][H]`, gate pre-activations `[tile][T][6][48][256]`; per layer ONE input GEMM over all tiles and ONE launch
-of the recurrent kernel (one 6-CTA cluster per 48-chunk tile, 11 clusters for 512 chunks), 15 launches per batch, issued by
+Width 384 (hac), the headline path (`forward_tiles`): activations tile-major `[tile][T][64][H]`, gate pre-activations
+`[tile][T][8][64][192]`; per layer ONE input GEMM over all tiles and ONE launch of the recurrent kernel (one 8-CTA
+cluster per 64-chunk tile, 8 clusters for 512 chunks), 15 launches per batch, issued by
 one C call (`b200_lstm_crf_fwd`) unless per-kernel events or intermediate activations are asked for.  Buffers are cached
 per (batch, chunk length, slot): `slot` selects one of several independent buffer sets, so that consecutive batches can
 be in flight on different streams (`score_batches`, bench.py).
 
 Other widths (`forward_tiled`): the generic `[T][N][4H]` layout and the `mma.sync` recurrent kernel, tiles of 32 chunks
-pipelined on per-tile streams; `B200_LSTM_TILE=0` sends width 384 down this path with the first-generation tcgen05 kernel
-(8-CTA clusters), `B200_TILE_STREAMS=1` gives the tile-layout path per-tile streams as well (the round-1 schedule).
+pipelined on per-tile streams; `B200_LSTM_TILE=0` sends width 384 down this path (8-CTA clusters), `B200_TILE_STREAMS=1` gives the tile-layout path per-tile streams as well (the round-1 schedule).
 """
 
 import torch
@@ -142,7 +141,7 @@ class LstmCrfPlan:
         H = self.hidden
         if native.lstm_cluster_size(H) == 0:
             raise UnsupportedModel(f"LSTM hidden size {H} has no native kernel")
-        # H = 384: second-generation recurrent kernel (48-chunk tiles, 6-CTA clusters, gx streamed through shared memory)
+        # H = 384: tile-layout recurrent kernel (64-chunk tiles, 8-CTA clusters, wgmma)
         self.tile = native.lstm_tile_chunks(H)            # 0: only the generic-layout kernel exists for this width
         self.tile_cs = native.lstm_tile_cluster(H)
         unit = torch.arange(H)
@@ -362,7 +361,7 @@ class LstmCrfPlan:
         return out
 
     # ------------------------------------------------------------------------------------------
-    # tile layout (H = 384): activations [tile][T][48][H], gate pre-activations [tile][T][6][48][256]
+    # tile layout (H = 384): activations [tile][T][64][H], gate pre-activations [tile][T][8][64][192]
     # ------------------------------------------------------------------------------------------
     def _tile_layout_buffers(self, N, L, slot=0):
         key = ("tiles", N, L, slot)
@@ -429,7 +428,7 @@ class LstmCrfPlan:
         x = x.to(device=self.device, dtype=torch.float16).contiguous()
         N, L = x.shape
         H, TB, CS = self.hidden, self.tile, self.tile_cs
-        CW = 4 * H // CS                     # gx columns per cluster rank (256)
+        CW = 4 * H // CS                     # gx columns per cluster rank (192)
         b = self._tile_layout_buffers(N, L, slot)
         T, Tp, Lp, nt = b["T"], b["Tp"], b["Lp"], b["nt"]
         if out is None:
@@ -481,7 +480,7 @@ class LstmCrfPlan:
                             act=self.act_l, lo=self.lo, hi=self.hi, rows_inner=TB, valid_inner=nb, stride_inner=T,
                             stride_outer=1, impl=gemm_impl, stream=st, max_ctas=max_ctas)
 
-        def gather(buf):            # [tile][T][48][H] -> [T][N][H]
+        def gather(buf):            # [tile][T][64][H] -> [T][N][H]
             return buf.permute(1, 0, 2, 3).reshape(T, nt * TB, H)[:, :N].clone()
 
         if not streams and events is None and not return_features and gemm_impl == native.GEMM_AUTO and not self.quantize \
@@ -569,7 +568,7 @@ class LstmCrfPlan:
             if tiled is None:
                 # Default: the layer-by-layer schedule (14 launches per batch).  With two batches in flight on two streams
                 # (score_batches, bench.py) it measured faster than per-tile streams (17.8 vs 18.8 ms per 512-chunk batch):
-                # the GEMMs / decode of one batch fill the 82 SMs the other batch's recurrent clusters leave free.
+                # the GEMMs / decode of one batch fill the SMs the other batch's recurrent clusters leave free.
                 tiled = (not return_features) and x.shape[0] > self.tile and os.environ.get("B200_TILE_STREAMS", "0") != "0"
             return self.forward_tiles(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features,
                                       streams=tiled, slot=slot)

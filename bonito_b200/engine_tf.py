@@ -4,10 +4,10 @@ Plan builder + executor for the transformer (sup v5) encoder:
     NamedSerial(conv = Serial[Convolution x5, Permute([0,2,1])], transformer_encoder = Stack[TransformerEncoderLayer x18],
                 upsample = LinearUpsample(x2), crf = LinearCRFEncoder(scale=5, permute=[1,0,2]))
 
-(`/root/reference/bonito/models/configs/dna_r10.4.1@v5.0.toml`, `bonito/transformer/model.py:82-154`).  Like the
+(`bonito/models/configs/dna_r10.4.1@v5.0.toml`, `bonito/transformer/model.py:82-154`).  Like the
 reference's `use_koi` rewrite it returns scores batch-first, `[N, 2T', C]` fp16 without the blank column.
 
-Schedule per batch: conv_first kernel (1->64), four convolutions as tcgen05 GEMMs over overlapping channels-last rows
+Schedule per batch: conv_first kernel (1->64), four convolutions as wgmma GEMMs over overlapping channels-last rows
 (swish in the epilogue, output written straight into the next layer's zero-haloed buffer), then per layer
 QKV GEMM -> rotary + windowed attention -> out-proj GEMM (+bias) -> residual RMSNorm -> fc1 GEMM -> SwiGLU -> fc2 GEMM ->
 residual RMSNorm, then the upsample GEMM (+bias; the x2 reshape is free in a batch-first layout) and the CRF GEMM (x scale).

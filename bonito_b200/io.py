@@ -1,6 +1,6 @@
 """
 pysam-free output for `bonito_b200 basecaller`: unaligned FASTQ and unaligned SAM text with the reference's header, record
-and tag layout (`/root/reference/bonito/io.py:41-166,400-469`, `/root/reference/documentation/SAM.md`), including the
+and tag layout (`bonito/io.py:41-166,400-469`, `documentation/SAM.md`), including the
 sequence-to-signal move table `mv:B:c,<stride>,<moves...>` (`io.py:57-70,455-456`).  The reference writes through
 pysam / htslib (and aligns with mappy); BAM / CRAM need htslib and alignment needs minimap2, neither of which this build
 bundles, so those formats are refused with an explanation instead of being approximated.

@@ -1,6 +1,6 @@
 """
 `thread_iter`: run an iterator on a background thread with a bounded queue, the only piece of
-`/root/reference/bonito/multiprocessing.py` (lines 20-24, 92-122) on the chunked GPU path.
+`bonito/multiprocessing.py` (lines 20-24, 92-122) on the chunked GPU path.
 """
 
 import queue

@@ -16,7 +16,7 @@ _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libbonito_
 _lib = None
 
 ACT_NONE, ACT_SWISH, ACT_TANH, ACT_CLAMP, ACT_SCALE, ACT_SWIGLU, ACT_TANH_SCALE = 0, 1, 2, 3, 4, 5, 6
-GEMM_AUTO, GEMM_TCGEN05, GEMM_MMA_SYNC, GEMM_TCGEN05_PAIR = 0, 1, 2, 3
+GEMM_AUTO, GEMM_TCGEN05, GEMM_MMA_SYNC = 0, 1, 2
 
 MAX_LSTM_LAYERS = 8
 
@@ -58,15 +58,6 @@ SIGNATURES = {
     "b200_lstm_tile_cluster": (c_int, [c_int]),
     "b200_lstm_rec_tile_workspace_bytes": (c_size_t, [c_int]),
     "b200_lstm_rec_tile_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "b200_debug_lstm_tile_timeline": (c_int, [c_void_p, c_int]),
-    "b200_debug_attention_timeline": (c_int, [c_void_p, c_int]),
-    "b200_debug_gemm_profile": (c_int, [c_void_p]),
-    "b200_debug_tmem_probe": (c_int, [c_void_p, c_void_p]),
-    "b200_debug_lstm_timeline": (c_int, [c_void_p, c_int]),
-    "b200_debug_lstm_max_clusters": (c_int, []),
-    "b200_debug_max_clusters": (c_int, [c_int, c_int, c_int]),
-    "b200_debug_exchange_bench": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    "b200_debug_mma_bench": (c_int, [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b200_crf_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_quantize_i8": (c_int, [c_void_p, c_void_p, c_longlong, c_float, c_void_p]),
     "b200_stream_create": (c_int, [c_void_p]),
@@ -111,7 +102,7 @@ def require(device=None):
     """Library + CUDA device, or a loud failure."""
     lib = load()
     if not torch.cuda.is_available():
-        raise NativeError("bonito_b200 native path needs a CUDA device (sm_100a); none is visible")
+        raise NativeError("bonito_b200 native path needs a CUDA device (sm_90a); none is visible")
     return lib
 
 
@@ -235,7 +226,7 @@ def lstm_rec_tile_workspace_bytes(n):
 
 
 def lstm_rec_tile(gx, whh, y, t, n, hidden, reverse, stream=None, workspace=None):
-    """gx [tiles][T][6][48][256], y [tiles][T][48][H] (see b200_lstm_rec_tile_fwd); n chunks = ceil(n/48) tiles.
+    """gx [tiles][T][8][64][192], y [tiles][T][64][H] (see b200_lstm_rec_tile_fwd); n chunks = ceil(n/64) tiles.
     `workspace`: uint8 tensor of lstm_rec_tile_workspace_bytes(n) bytes (allocated here when omitted)."""
     lib = require()
     if workspace is None:
@@ -245,45 +236,6 @@ def lstm_rec_tile(gx, whh, y, t, n, hidden, reverse, stream=None, workspace=None
                                         int(bool(reverse)), _stream(stream))
     _check(rc, "b200_lstm_rec_tile_fwd")
     return y
-
-
-def lstm_tile_timeline(steps=256):
-    """[steps, 8] int64 SM-clock stamps recorded by CTA 0 of the last lstm_rec_tile launch under B200_LSTM_DEBUG=3."""
-    import numpy as np
-    buf = np.zeros((steps, 8), dtype=np.int64)
-    n = load().b200_debug_lstm_tile_timeline(buf.ctypes.data_as(c_void_p), steps)
-    if n < 0:
-        _check(n, "b200_debug_lstm_tile_timeline")
-    return buf[:n]
-
-
-def tmem_probe():
-    """Run the TMEM convention probe; returns a float32 CPU tensor of 16384 values."""
-    lib = require()
-    out = torch.zeros(16384, dtype=torch.float32, device="cuda")
-    rc = lib.b200_debug_tmem_probe(_ptr(out), _stream())
-    _check(rc, "b200_debug_tmem_probe")
-    torch.cuda.synchronize()
-    return out.cpu()
-
-
-def mma_bench(ts_mode, n, iters=960, chains=1, blocks=1):
-    """(issue cycles, issue-to-completion cycles, ns) of tcgen05.mma M=128 x N=n x K=16 over `chains` accumulators."""
-    lib = require()
-    out = torch.zeros(3, dtype=torch.int64, device="cuda")
-    _check(lib.b200_debug_mma_bench(int(ts_mode), n, iters, chains, blocks, _ptr(out), _stream()), "b200_debug_mma_bench")
-    torch.cuda.synchronize()
-    return out.cpu().tolist()
-
-
-def lstm_timeline(steps=256):
-    """[steps, 8] int64 SM-clock stamps recorded by CTA 0 of the last lstm_rec launch under B200_LSTM_DEBUG=3."""
-    import numpy as np
-    buf = np.zeros((steps, 8), dtype=np.int64)
-    n = load().b200_debug_lstm_timeline(buf.ctypes.data_as(c_void_p), steps)
-    if n < 0:
-        _check(n, "b200_debug_lstm_timeline")
-    return buf[:n]
 
 
 def crf_decode_workspace_bytes(n, t, state_len):

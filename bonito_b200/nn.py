@@ -2,15 +2,15 @@
 Layer registry for bonito_b200 -- the host-side mirror of `bonito.nn`.
 
 This module keeps the reference's plugin surface for the chunked forward path
-(`/root/reference/bonito/nn.py:13-19` registry, `:418-444` to_dict/from_dict,
+(`bonito/nn.py:13-19` registry, `:418-444` to_dict/from_dict,
 `:447-454` fuse_bn_) so that model `config.toml` files written for the reference
 build the same module tree here, with the same `state_dict()` key names and
-shapes (`match_names`, `/root/reference/bonito/util.py:239-248`, pairs
+shapes (`match_names`, `bonito/util.py:239-248`, pairs
 checkpoints to modules by sorted shape).
 
 The torch modules in this file are *descriptions plus parameter storage*: the
-B200 engine (`bonito_b200.engine`) walks the tree, packs the weights and runs
-the hand-written sm_100a kernels.  `forward()` on the individual layers is a
+native engine (`bonito_b200.engine`) walks the tree, packs the weights and runs
+the hand-written sm_90a kernels.  `forward()` on the individual layers is a
 plain-torch definition of the layer semantics, used on CPU by the host-logic
 tests; it is never the product path on a GPU box (see `bonito_b200.crf.model`).
 """

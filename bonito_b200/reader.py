@@ -1,7 +1,7 @@
 """
 Read ingestion for `bonito_b200 basecaller`.
 
-The reference picks a pod5 or fast5 reader by globbing the reads directory (`/root/reference/bonito/reader.py:23-48`);
+The reference picks a pod5 or fast5 reader by globbing the reads directory (`bonito/reader.py:23-48`);
 both need third-party libraries (pod5, ont_fast5_api) that are optional here.  Supported inputs:
   * `*.pod5`  through the `pod5` package when it is importable (signal in pA = scale * (raw + offset));
   * `*.npy`   one read per file: a 1-D array of picoampere samples, read id = file stem (what the tests and the

@@ -2,10 +2,10 @@
 Synthetic LSTM-CRF / transformer models and signals (a utility of the package: no kernel or oracle code in here).
 
 There is no network in the build environment, so the real `dna_r10.4.1_e8.2_400bps_{fast,hac}@v5.0.0`
-checkpoints cannot be fetched (`/root/reference/bonito/cli/download.py:31-83`); every test and benchmark uses
+checkpoints cannot be fetched (`bonito/cli/download.py:31-83`); every test and benchmark uses
 seeded random weights of the same architecture (shapes: SURVEY.md Appendix A), stored in the reference's own
 on-disk format (`config.toml` + `weights_1.tar`) so the same files drive the reference modules, the oracle
-and the B200 engine.
+and the native engine.
 """
 
 import os
@@ -150,7 +150,7 @@ def gaussian_signal(n, length, seed=25):
 
 
 # ---------------------------------------------------------------------------------------------------
-# transformer (sup v5.0) shapes: /root/reference/bonito/models/configs/dna_r10.4.1@v5.0.toml
+# transformer (sup v5.0) shapes: bonito/models/configs/dna_r10.4.1@v5.0.toml
 # ---------------------------------------------------------------------------------------------------
 
 def sup_spec(depth=18, d_model=512, nhead=8, dim_feedforward=2048, state_len=5):

@@ -1,11 +1,11 @@
 """
-Transformer (sup v5) model package -- host-side mirror of `/root/reference/bonito/transformer/model.py`.
+Transformer (sup v5) model package -- host-side mirror of `bonito/transformer/model.py`.
 
 The reference builds its layer from flash-attn modules (`RotaryEmbedding`, `GatedMlp`, Triton `RMSNorm`,
 `flash_attn_qkvpacked_func`); here the same parameters (same `state_dict` names and shapes) sit in plain torch
 modules whose `forward` spells out the arithmetic those kernels implement (flash-attn's own torch reference
-functions: `rms_norm_ref`, `apply_rotary_emb_torch`, `swiglu_fwd`).  With `use_koi` armed the B200 engine
-(`bonito_b200.engine_tf`) runs the stack on the sm_100a kernels instead.
+functions: `rms_norm_ref`, `apply_rotary_emb_torch`, `swiglu_fwd`).  With `use_koi` armed the native engine
+(`bonito_b200.engine_tf`) runs the stack on the sm_90a kernels instead.
 """
 
 import types

@@ -1,7 +1,7 @@
 """
 Host-side helpers of the chunked basecalling path: chunk / stitch / batchify /
 unbatchify and the model loader.  Semantics follow the reference bit for bit
-(`/root/reference/bonito/util.py:142-311`); the tests in `tests/test_host_logic.py`
+(`bonito/util.py:142-311`); the tests in `tests/test_host_logic.py`
 replay the known answers recorded in SURVEY.md Appendix A and the golden
 fixtures generated from the reference's own functions.
 """
@@ -33,7 +33,7 @@ except ImportError:  # pragma: no cover - python >= 3.11 always has tomllib
 __dir__ = Path(__file__).parent
 __models_dir__ = __dir__ / "models"
 
-# model packages named in reference configs resolve to their B200 counterparts
+# model packages named in reference configs resolve to their native counterparts
 _PACKAGE_ALIASES = {
     "bonito.crf": "bonito_b200.crf",
     "bonito.transformer": "bonito_b200.transformer",

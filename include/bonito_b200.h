@@ -1,5 +1,5 @@
 /*
- * bonito_b200 -- C ABI of the B200-native chunked forward + decode path.
+ * bonito_b200 -- C ABI of the H100-native (sm_90a) chunked forward + decode path.
  *
  * The reference (nanoporetech/bonito) is pure Python; its native work on this path is done by
  * third-party binaries reached from these call sites, which are what each entry point replaces:
@@ -33,17 +33,16 @@ extern "C" {
 #define B200_ACT_TANH 2
 #define B200_ACT_CLAMP 3 /* clamp(lo, hi), Clamp layer: bonito/nn.py:59-67 */
 #define B200_ACT_SCALE 4 /* multiply by lo, LinearCRFEncoder.scale: bonito/nn.py:288-289 */
-/* SwiGLU fused into the GEMM (tcgen05 path only): the n output columns are 64-wide groups [32 x y | 32 x gate] (the caller
+/* SwiGLU fused into the GEMM (wgmma path only): the n output columns are 64-wide groups [32 x y | 32 x gate] (the caller
  * interleaves the rows of fc1.weight that way) and c receives n/2 columns, c[:, 32*g + j] = gate * y / (1 + exp(-gate)) on the
  * fp16-rounded y / gate, rounded once -- GatedMlp: flash_attn/modules/mlp.py:99-136, flash_attn/ops/activations.py:107-111
  * as used by bonito/transformer/model.py:100-104.  n % 64 == 0, no bias. */
 #define B200_ACT_SWIGLU 5
 #define B200_ACT_TANH_SCALE 6 /* tanh, then multiply by lo: LinearCRFEncoder(activation="tanh", scale=5.0), bonito/nn.py:283-298 */
 
-#define B200_GEMM_AUTO 0 /* tcgen05 (product path) unless B200_GEMM_IMPL=mma is set in the environment */
-#define B200_GEMM_TCGEN05 1
+#define B200_GEMM_AUTO 0 /* the wgmma kernel (product path) unless B200_GEMM_IMPL=mma is set in the environment */
+#define B200_GEMM_TCGEN05 1 /* the wgmma kernel (the name is kept for ABI compatibility) */
 #define B200_GEMM_MMA_SYNC 2 /* legacy tensor path, kept for on-device cross-checks */
-#define B200_GEMM_TCGEN05_PAIR 3 /* cta_group::2 pair kernels (N % 256 == 0): faster alone, not the default next to other kernels */
 
 /* Library version (major*10000 + minor*100 + patch). */
 int b200_version(void);
@@ -77,8 +76,7 @@ int b200_gemm_fwd(const void* a, long long lda, const void* b, const void* bias,
 
 /*
  * Same, with
- *   max_ctas  a cap on the number of (persistent) CTAs the tcgen05 kernel may occupy (0 = every SM): the tile-pipelined
- *             engine caps the GEMMs it runs next to resident recurrent clusters;
+ *   max_ctas  accepted for compatibility and ignored: the wgmma kernel is not persistent (its CTAs leave as they finish);
  *   group, stride_group  second level of the row map (group = 0: off): (outer2, outer1) = divmod(outer, group),
  *             out_row = inner*stride_inner + outer1*stride_outer + outer2*stride_group -- e.g. chunk n -> (tile n/48, n%48);
  *   cb_width, cb_rows  column blocks (cb_width = 0: off; multiple of 32): output column c of mapped row R is written to
@@ -103,40 +101,30 @@ int b200_lstm_cluster_size(int hidden);
  *   whh [4H][H]     recurrent weights, rows permuted to [cluster rank][unit/8 block][gate][unit%8]
  *   y   [T][N][H]   h_t in natural unit order
  * reverse != 0 runs t = T-1..0 (the reference flips the sequence instead: bonito/nn.py:366-370).
- * hidden = 384 runs the tcgen05 kernel (W_hh resident in tensor memory, h exchanged through distributed shared
- * memory); other sizes, or B200_LSTM_IMPL=mma in the environment, run the mma.sync kernel.
+ * Every supported size runs the mma.sync kernel (W_hh resident in shared memory, h exchanged through L2); the hot path of
+ * hidden = 384 is the tile-layout kernel below.
  */
 int b200_lstm_rec_fwd(const void* gx, const void* whh, void* y, int t, int n, int hidden, int reverse,
                       void* stream);
 
 /*
- * Tile layout of the H = 384 recurrent kernel (second generation: clusters of 6 CTAs x 64 hidden units, three interleaved
- * 16-chunk sub-tiles, input projection streamed through shared memory by cp.async.bulk).
- *   b200_lstm_tile_chunks(hidden)   chunks per tile (48 for hidden = 384; 0 = this hidden size has no tile kernel)
- *   b200_lstm_tile_cluster(hidden)  CTAs per cluster = column blocks of gx (6)
- *   gx  [tiles][T][6][48][256]  columns of cluster rank r: [unit/8 - 8r][unit%8][gate i,f,g,o]  (b200_gemm_fwd_ex with
- *                               rows (t, chunk), cb_width = 256, cb_rows = 48, ldc = 256)
+ * Tile layout of the H = 384 recurrent kernel (clusters of 8 CTAs x 48 hidden units, W_hh slice resident in shared memory,
+ * wgmma on 64-chunk tiles, h all-gather as multicast bulk copies through L2).
+ *   b200_lstm_tile_chunks(hidden)   chunks per tile (64 for hidden = 384; 0 = this hidden size has no tile kernel)
+ *   b200_lstm_tile_cluster(hidden)  CTAs per cluster = column blocks of gx (8)
+ *   gx  [tiles][T][8][64][192]  columns of cluster rank r: [unit - 48r][gate i,f,g,o]  (b200_gemm_fwd_ex with
+ *                               rows (t, chunk), cb_width = 192, cb_rows = 64, ldc = 192)
  *   whh [4H][H]                 as for b200_lstm_rec_fwd
- *   y   [tiles][T][48][H]       h_t in natural unit order; rows of chunks >= n are not written
- *   workspace                   b200_lstm_rec_tile_workspace_bytes(n) bytes (72 KB per tile): staging of the h all-gather,
- *                               which goes through L2 as multicast bulk copies; contents irrelevant, but launches that
- *                               may run concurrently need distinct workspaces
- * tiles = ceil(n / 48); one launch runs all of them (one cluster each; 22 fit on a B200 at once).
+ *   y   [tiles][T][64][H]       h_t in natural unit order; rows of chunks >= n are not written
+ *   workspace                   b200_lstm_rec_tile_workspace_bytes(n) bytes (96 KB per tile): staging of the h all-gather;
+ *                               contents irrelevant, but launches that may run concurrently need distinct workspaces
+ * tiles = ceil(n / 64); one launch runs all of them (one cluster each).
  */
 int b200_lstm_tile_chunks(int hidden);
 int b200_lstm_tile_cluster(int hidden);
 size_t b200_lstm_rec_tile_workspace_bytes(int n);
 int b200_lstm_rec_tile_fwd(const void* gx, const void* whh, void* y, void* workspace, int t, int n, int hidden,
                            int reverse, void* stream);
-
-/* Timing aid: after a b200_attention_fwd launched with B200_ATTN_DEBUG=1, the SM-clock stamps CTA 0 recorded for its first
- * query tiles ([tile][16] int64, HOST buffer; see attention_tc.cu).  Returns the number of tiles copied (<= 64). */
-int b200_debug_attention_timeline(long long* host_out, int max_tiles);
-/* B200_GEMM_DEBUG=1: per-CTA cycle counters of the last weight-stationary GEMM launch, 160 x 8 values (gemm_tc.cu) */
-int b200_debug_gemm_profile(long long* host_out);
-
-/* Timing aid: as b200_debug_lstm_timeline, for b200_lstm_rec_tile_fwd. */
-int b200_debug_lstm_tile_timeline(long long* host_out, int max_steps);
 
 /*
  * ---- transformer (sup) path: bonito/transformer/model.py ----
@@ -162,42 +150,6 @@ int b200_rmsnorm_residual_fwd(const void* a, const void* x, const void* w, float
 
 /* h [m][2f] = (y | gate) -> out [m][f] = gate * y / (1 + exp(-gate))   (GatedMlp with SiLU). */
 int b200_swiglu_fwd(const void* h, void* out, long long m, int f, void* stream);
-
-/*
- * Self-test of the tensor-memory conventions the tcgen05 kernels rely on (fragment layout of
- * tcgen05.ld.16x256b, fp16-pair packing of a TMEM-resident A operand, un-swizzled B tiles).  out: 16384 floats (device);
- * interpreted by tests/test_gpu_kernels.py::test_tmem_conventions.
- */
-int b200_debug_tmem_probe(void* out, void* stream);
-
-/* Number of 8-CTA clusters of the tcgen05 recurrent kernel the current device can hold at once (-1 on error). */
-int b200_debug_lstm_max_clusters(void);
-
-/*
- * Timing aid: the h all-gather of the tile recurrent kernel without the math (6-CTA clusters, 3 x 8 sender warps per CTA,
- * 256-byte blocks into the h tiles of all six CTAs every step; see debug_bench.cu for the modes: 0 DSMEM bulk copies,
- * 2 / 3 multicast bulk copies out of an L2 staging buffer, 4 DSMEM with 2 KB copies).  staging: clusters * 73728 bytes
- * (device); out: 2 x int64 (device) = cycles of CTA 0, steps.
- */
-int b200_debug_exchange_bench(int mode, int steps, int delay, int clusters, void* staging, void* out, void* stream);
-
-/* Occupancy query: clusters of `cluster_size` CTAs (`threads` threads, `smem_bytes` dynamic shared memory, one CTA per SM
- * when smem_bytes > half an SM) the current device holds at once; -1 on error.  GPC packing decides (B200: 148 SMs). */
-int b200_debug_max_clusters(int cluster_size, int threads, int smem_bytes);
-
-/*
- * Timing aid: after a b200_lstm_rec_fwd launched with B200_LSTM_DEBUG=3 in the environment, copies the SM-clock
- * stamps CTA 0 recorded for its first steps ([step][8] int64, HOST buffer; see lstm_rec_tc.cu).  Returns the
- * number of steps copied (<= 256) or a negative error.
- */
-int b200_debug_lstm_timeline(long long* host_out, int max_steps);
-
-/*
- * Timing aid: `iters` tcgen05.mma (M=128, N=n, K=16, fp16) round-robin over `chains` independent accumulators, A from
- * tensor memory (ts_mode=1) or shared memory (0), on `blocks` CTAs; out (device, 3 x int64): issue cycles,
- * issue-to-completion cycles, nanoseconds.
- */
-int b200_debug_mma_bench(int ts_mode, int n, int iters, int chains, int blocks, void* out, void* stream);
 
 /* Bytes of scratch b200_crf_decode needs for n chunks of t frames. */
 size_t b200_crf_decode_workspace_bytes(int n, int t, int state_len);
@@ -235,8 +187,8 @@ int b200_stream_create(void** stream_out);
  * ---- INT8 input projection (--quantize; reference: koi's int8 LSTM path, bonito/crf/model.py:245, cli/basecaller.py:186-189) ----
  * b200_quantize_i8: out[i] = clamp(rint(x[i] * scale), -127, 127), fp16 -> int8, n a multiple of 8.
  * b200_gemm_i8_fwd: C = act(col_scale[j] * sum_k A_i8[i][k] B_i8[j][k] + bias[j]) -- int8 operands (lda in bytes), s32
- *   accumulation on tcgen05 kind::i8, per-column float scale (weight scale / activation scale), fp16 bias / output, the
- *   same row / column-block maps as b200_gemm_fwd_ex.  K <= 768, K % 16 == 0, N a multiple of 192 or 128.
+ *   accumulation on the int8 tensor cores (wgmma s8), per-column float scale (weight scale / activation scale), fp16 bias /
+ *   output, the same row / column-block maps as b200_gemm_fwd_ex.  K % 16 == 0, N % 8 == 0.
  */
 int b200_quantize_i8(const void* x, void* out, long long n, float scale, void* stream);
 int b200_gemm_i8_fwd(const void* a, long long lda, const void* b, const void* col_scale, const void* bias, void* c,

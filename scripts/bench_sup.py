@@ -1,4 +1,4 @@
-"""Timing of BASELINE config 3: sup v5.0-shaped transformer (18 layers, d=512), batch 256, 9996-sample chunks, 1 GPU."""
+"""Timing of benchmark config 3: sup v5.0-shaped transformer (18 layers, d=512), batch 256, 9996-sample chunks, 1 GPU."""
 import os, sys, json
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

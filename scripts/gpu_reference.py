@@ -1,6 +1,6 @@
 """
 Same-box GPU reference timing (SURVEY.md section 8d): the reference's PyTorch GPU execution of the forward pass, rebuilt from
-the library pieces the reference itself uses, timed beside the sm_100a path on identical weights and input.
+the library pieces the reference itself uses, timed beside the sm_90a path on identical weights and input.
 
   hac / fast : torch.nn.Conv1d + SiLU/tanh, torch.nn.LSTM (cuDNN, fp16) with flips, Linear + clamp -- the module tree
                bonito.nn builds with use_koi=False (bonito/nn.py:221-241,353-415,268-298).

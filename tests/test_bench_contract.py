@@ -1,5 +1,5 @@
-"""The committed bench lines (profiles/) carry every key of the bench.py contract -- a guard against drifting away from
-what the driver parses.  CPU only: it reads the JSON written by the last GPU run."""
+"""The committed bench lines (profiles/) carry every key of the bench.py output format -- a guard against drifting away
+from what consumers of the line parse.  CPU only: it reads the JSON written by the last GPU run."""
 import json
 import os
 
@@ -15,7 +15,7 @@ def _last_json_line(path):
 
 
 def test_committed_bench_line_has_the_contract_keys():
-    d = _last_json_line(os.path.join(ROOT, "profiles", "r02_bench.json"))
+    d = _last_json_line(os.path.join(ROOT, "profiles", "h100_bench.json"))
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
                 "vs_baseline", "dtype", "data", "config", "e2e", "gpu_launches", "roofline", "cpu_baseline", "clocks"):
         assert key in d, key
@@ -32,7 +32,7 @@ def test_committed_bench_line_has_the_contract_keys():
     for key in ("sm_mhz", "sm_max_mhz", "reasons"):
         assert key in d["clocks"], key
     assert not set(d["clocks"]["reasons"]) & {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
-    # BASELINE configs 3, 5 and 1 and the --quantize configuration ride on the same line
+    # configs 3, 5 and 1 and the --quantize configuration ride on the same line
     cfg = d["configs"]
     for key in ("value", "unit", "ms_per_step", "e2e", "roofline", "stage_ms_per_step", "gpu_launches"):
         assert key in cfg["config3_sup"], key
@@ -41,7 +41,7 @@ def test_committed_bench_line_has_the_contract_keys():
 
 
 def test_committed_reference_arm_line():
-    d = _last_json_line(os.path.join(ROOT, "profiles", "r02_bench_reference.json"))
+    d = _last_json_line(os.path.join(ROOT, "profiles", "h100_bench_reference.json"))
     assert d["impl"] == "reference" and d["cpu_baseline"]["kind"] in ("port", "reference")
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
     assert d["e2e"]["value"] == d["value"] and d["unit"] == "samples/s"

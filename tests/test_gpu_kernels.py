@@ -129,9 +129,10 @@ def test_lstm_layer_matches_oracle(native, hidden, n, t, reverse):
 
 @pytest.mark.parametrize("impl_name", ["tcgen05", "mma"])
 def test_gemm_column_blocks(native, impl_name):
-    """cb_width / cb_rows: the layout the tile recurrent kernel reads, [t][rank][chunk][256] from rows (t, chunk)."""
+    """cb_width / cb_rows: the layout the tile recurrent kernel reads, [t][rank][chunk][cw] from rows (t, chunk)."""
     impl = native.GEMM_TCGEN05 if impl_name == "tcgen05" else native.GEMM_MMA_SYNC
-    t, tb, cs, cw, k = 37, 48, 6, 256, 384
+    t, tb, cs, k = 37, native.lstm_tile_chunks(384), native.lstm_tile_cluster(384), 384
+    cw = 4 * 384 // cs
     g = torch.Generator().manual_seed(11)
     a = _dev(torch.randn(t * tb, k, generator=g))
     w = _dev(torch.randn(cs * cw, k, generator=g) / k ** 0.5)
@@ -148,11 +149,11 @@ def test_gemm_column_blocks(native, impl_name):
 @pytest.mark.parametrize("n,t,reverse", [(5, 30, False), (16, 1, True), (17, 2, False), (48, 3, True), (50, 31, False),
                                          (100, 12, True), (96, 40, False), (33, 9, True)])
 def test_lstm_tile_kernel_matches_oracle(native, n, t, reverse):
-    """Second-generation H=384 recurrent kernel (6-CTA clusters, 48-chunk tiles, gx through the shared-memory ring): whole,
-    partial and multiple tiles, 1..3 active sub-tiles, T below / above the ring depth, both directions."""
+    """Tile-layout H=384 recurrent kernel (8-CTA clusters, 64-chunk tiles, wgmma, multicast h exchange): whole, partial and
+    multiple tiles, T = 1 .. 40, both directions."""
     H = 384
     tb, cs = native.lstm_tile_chunks(H), native.lstm_tile_cluster(H)
-    assert (tb, cs) in ((48, 6), (64, 6))       # B200_LSTM_SHAPE=3x16 (default) / 2x32
+    assert (tb, cs) == (64, 8)
     cw = 4 * H // cs
     nt = -(-n // tb)
     g = torch.Generator().manual_seed(1000 + n + t)
@@ -180,7 +181,7 @@ def test_lstm_tile_kernel_matches_oracle(native, n, t, reverse):
     assert torch.isnan(got[:, n:]).all()          # rows of chunks beyond the batch are not written
     err = (got[:, :n] - ref).abs().max().item()
     assert err <= 5e-3, err
-    # the two kernels agree to the rounding of h: same MMA shapes and accumulation order -> bitwise
+    # the two kernels agree to the rounding of h: same cell math, fp32 accumulation of the same fp16 products -> bitwise
     gx_old = torch.empty(t, n, 4 * H, dtype=torch.float16, device="cuda")
     native.gemm(_dev(x), H, _dev(w_ih[perm_ih]), _dev(b[perm_ih]), gx_old, 4 * H, t * n, 4 * H, H)
     y_old = torch.empty(t, n, H, dtype=torch.float16, device="cuda")
@@ -192,20 +193,19 @@ def test_lstm_tile_kernel_matches_oracle(native, n, t, reverse):
 @pytest.mark.parametrize("m,n,k,colblocks,act", [(48 * 431, 1536, 384, True, None), (128 * 70 + 33, 4096, 384, False, "clamp"),
                                                   (256 * 40, 512, 320, False, "tanh"), (128 * 81 + 5, 1536, 512, False, None),
                                                   (256 * 33, 512, 2048, False, None)])
-@pytest.mark.parametrize("impl_name", ["auto", "pair"])
+@pytest.mark.parametrize("impl_name", ["auto", "mma"])
 def test_gemm_many_row_blocks(native, impl_name, m, n, k, colblocks, act):
-    """Shapes of the headline batch's GEMMs with enough rows (>= 64 row blocks) for the weight-stationary kernels and, when N
-    is a multiple of 256, the cta_group::2 pair kernels (impl "pair": weight-stationary for K <= 384, streaming beyond):
-    every output element against fp32 matmul of the same operands."""
+    """Shapes of the headline batch's GEMMs with many row blocks, on the wgmma kernel (auto) and the mma.sync kernel: every
+    output element against fp32 matmul of the same operands."""
     g = torch.Generator().manual_seed(m % 1000 + n)
     a = (torch.randn(m, k, generator=g) * 0.5).half()
     w = (torch.randn(n, k, generator=g) / k ** 0.5).half()
     bias = torch.randn(n, generator=g).half()
     ref = _ref_gemm(a, w, bias, act, -5.0, 5.0)
     act_code = {None: native.ACT_NONE, "clamp": native.ACT_CLAMP, "tanh": native.ACT_TANH}[act]
-    impl = native.GEMM_TCGEN05_PAIR if impl_name == "pair" else native.GEMM_AUTO
+    impl = native.GEMM_MMA_SYNC if impl_name == "mma" else native.GEMM_AUTO
     if colblocks:
-        tb, cs, cw = 48, 6, 256
+        tb, cs, cw = 48, 6, 256     # any column-block geometry: 48 * 431 rows, 1536 = 6 x 256 columns
         out = torch.full((m // tb, cs, tb, cw), float("nan"), dtype=torch.float16, device="cuda")
         native.gemm(_dev(a), k, _dev(w), _dev(bias), out, cw, m, n, k, act=act_code, rows_inner=tb, valid_inner=tb, stride_inner=1,
                     stride_outer=cs * tb, cb_width=cw, cb_rows=tb, impl=impl)
@@ -222,7 +222,7 @@ def test_gemm_many_row_blocks(native, impl_name, m, n, k, colblocks, act):
 @pytest.mark.parametrize("m,n,k,bias,cb", [(1000, 1536, 384, True, False), (4096 + 77, 384, 256, False, False),
                                            (37 * 48, 1536, 384, True, True)])
 def test_gemm_int8_matches_integer_matmul(native, m, n, k, bias, cb):
-    """tcgen05 kind::i8: exact s32 accumulation of int8 products, per-column scale and bias in the epilogue."""
+    """wgmma s8: exact s32 accumulation of int8 products, per-column scale and bias in the epilogue."""
     g = torch.Generator().manual_seed(m + n)
     a = torch.randint(-127, 128, (m, k), generator=g, dtype=torch.int8)
     w = torch.randint(-127, 128, (n, k), generator=g, dtype=torch.int8)
@@ -269,44 +269,13 @@ def test_quantize_i8(native):
     assert torch.equal(out.cpu(), want)
 
 
-def test_tmem_conventions(native):
-    """tcgen05.ld.16x256b fragment layout and the fp16-pair packing of a TMEM-resident A operand."""
-    out = native.tmem_probe().numpy()
-    frag = out[:4096].reshape(128, 32)
-    tid = np.arange(128)
-    warp, lane = tid // 32, tid % 32
-    want = np.zeros((128, 32), dtype=np.float32)
-    for half in range(2):
-        for j in range(4):
-            for hi in range(2):
-                for e in range(2):
-                    row = warp * 32 + 16 * half + lane // 4 + 8 * hi
-                    col = 8 * j + 2 * (lane % 4) + e
-                    want[:, 16 * half + 4 * j + 2 * hi + e] = 100 * row + col
-    if not np.array_equal(frag, want):
-        print("observed fragment of thread 0..7:\n", frag[:8])
-    assert np.array_equal(frag, want)
-    d = out[4096:8192].reshape(128, 32)
-    i, n, k = np.arange(128)[:, None, None], np.arange(32)[None, :, None], np.arange(16)[None, None, :]
-    ref = ((((i % 7) + k) * 0.25) * (((n + k) % 5) * 0.5)).sum(-1)
-    if not np.allclose(d, ref, atol=1e-3):
-        print("observed D[0:4, 0:8]:\n", d[:4, :8], "\nexpected:\n", ref[:4, :8])
-    np.testing.assert_allclose(d, ref, atol=1e-3)
-    # un-swizzled K-major B tile: leading byte offset = K direction, stride byte offset = 8-row groups
-    ns_a, ns_b = out[8192:12288].reshape(128, 32), out[12288:].reshape(128, 32)
-    print("no-swizzle (lbo=K, sbo=rows) matches:", np.allclose(ns_a, ref, atol=1e-3),
-          "; swapped matches:", np.allclose(ns_b, ref, atol=1e-3))
-    np.testing.assert_allclose(ns_a, ref, atol=1e-3)
-
-
-@pytest.mark.parametrize("impl", ["tcgen05", "mma"])
+@pytest.mark.parametrize("impl", ["tile", "mma"])
 @pytest.mark.parametrize("n,t,reverse", [(7, 30, False), (40, 12, True), (64, 50, False), (33, 3, True)])
-def test_lstm_384_both_kernels(native, monkeypatch, impl, n, t, reverse):
-    if impl == "mma":
-        monkeypatch.setenv("B200_LSTM_IMPL", "mma")
+def test_lstm_384_both_kernels(native, impl, n, t, reverse):
+    if impl == "tile":
+        test_lstm_tile_kernel_matches_oracle(native, n, t, reverse)
     else:
-        monkeypatch.delenv("B200_LSTM_IMPL", raising=False)
-    test_lstm_layer_matches_oracle(native, 384, n, t, reverse)
+        test_lstm_layer_matches_oracle(native, 384, n, t, reverse)
 
 
 @pytest.mark.parametrize("state_len,n,t", [(3, 4, 200), (4, 3, 333), (4, 2, 1666), (5, 2, 60), (3, 1, 1), (4, 2, 2), (3, 3, 7),

@@ -22,7 +22,7 @@ def _model(name, n_lstm=5, seed=25, batchnorm=False):
     return model.half().eval().to("cuda"), spec, weights
 
 
-# Tolerances.  BASELINE.json asks for "1e-3 fp16 tolerance": fp16 carries 11 significant bits, so one ulp of a score
+# Tolerances.  The target is a "1e-3 fp16 tolerance": fp16 carries 11 significant bits, so one ulp of a score
 # of magnitude 4..8 is 3.9e-3 and 1e-3 is a RELATIVE bound (~1 ulp).  Against the oracle run with the same fp16
 # storage rounding points the engine must stay within a few ulp (accumulation order differs); against the pure
 # fp32 oracle the bound is what half-precision storage of 7 stacked layers costs any implementation.
@@ -57,7 +57,7 @@ def test_forward_scores_match_oracle(name, n, L):
 @pytest.mark.parametrize("n", [33, 70, 128])
 def test_tile_pipelined_forward_is_bit_identical(n, monkeypatch):
     """Per-tile streams (the default for batches above one tile) vs the single-stream layer-by-layer schedule, and the
-    second-generation recurrent kernel (48-chunk tiles, default) vs the first (32-chunk tiles, B200_LSTM_TILE=0)."""
+    tile-layout recurrent kernel (64-chunk tiles, default) vs the generic-layout one (32-chunk tiles, B200_LSTM_TILE=0)."""
     model, spec, _ = _model("hac", n_lstm=3)
     x = synth.squiggle(n, 1200, seed=n).half().cuda()
     plan = model.native_plan("cuda")
@@ -159,7 +159,7 @@ def test_decode_of_own_scores_is_exact():
 
 def test_headline_shape_scores_and_sequences_match_oracle():
     """
-    BASELINE config 2 at full size: hac, batch 512 x 9996 samples (T = 1666), 64 distinct chunks repeated 8 times.
+    Benchmark config 2 at full size: hac, batch 512 x 9996 samples (T = 1666), 64 distinct chunks repeated 8 times.
     16 chunks spread over the batch (different tiles, different copies) are compared with the CPU oracle run with the
     same fp16 storage rounding: scores within fp16 tolerance (north star: 1e-3 relative; one fp16 ulp at |x| in [4, 8)
     is 3.9e-3, the budget is two), and the base sequences of CUDA forward + CUDA decode against oracle forward + oracle
@@ -208,7 +208,7 @@ def test_headline_shape_scores_and_sequences_match_oracle():
 
 
 def test_full_size_properties():
-    """BASELINE config 2 (hac, batch 512, 9996 samples): determinism and chunk independence."""
+    """Benchmark config 2 (hac, batch 512, 9996 samples): determinism and chunk independence."""
     from bonito_b200.decode import beam_search
     model, spec, _ = _model("hac")
     x = synth.squiggle(64, 9996, seed=1).half()

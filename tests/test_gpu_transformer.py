@@ -43,6 +43,39 @@ def test_attention_matches_oracle(native, n, t, window):
     assert err <= 6e-3, err   # P is rounded to fp16 before the second product (as in flash-attn)
 
 
+@pytest.mark.parametrize("n,t,window", [(2, 1666, (127, 128)), (1, 300, (127, 128)), (2, 257, (0, 128)), (1, 400, (127, 0))])
+def test_attention_wgmma_and_mma_kernels_match_oracle(native, monkeypatch, n, t, window):
+    """The wgmma kernel (default) and the mma.sync kernel (B200_ATTN_IMPL=mma) on the sup window shapes: both against the
+    oracle, and against each other to the rounding of the output."""
+    g = torch.Generator().manual_seed(t + 7)
+    nh, hd = 8, 64
+    qkv = (torch.randn(n, t, 3, nh, hd, generator=g) * 1.5).half()
+    cos, sin = TO.rotary_tables(t, hd, fp16=True)
+    cs = _dev(torch.cat([cos, sin], dim=1))
+    outs = {}
+    for impl in ("wgmma", "mma"):
+        if impl == "mma":
+            monkeypatch.setenv("B200_ATTN_IMPL", "mma")
+        else:
+            monkeypatch.delenv("B200_ATTN_IMPL", raising=False)
+        out = torch.full((n, t, nh * hd), float("nan"), dtype=torch.float16, device="cuda")
+        native.attention(_dev(qkv), cs, out, n, t, nh, hd, window[0], window[1])   # a fresh copy: q, k are rotated in place
+        torch.cuda.synchronize()
+        outs[impl] = out.float().cpu()
+    x = qkv.float()
+    q = TO._r16(TO.apply_rotary(x[:, :, 0], cos, sin), True).permute(0, 2, 1, 3)
+    k = TO._r16(TO.apply_rotary(x[:, :, 1], cos, sin), True).permute(0, 2, 1, 3)
+    v = x[:, :, 2].permute(0, 2, 1, 3)
+    att = (q @ k.transpose(-1, -2)) / hd ** 0.5
+    att = att.masked_fill(~TO.window_mask(t, window), float("-inf"))
+    ref = (torch.softmax(att, dim=-1) @ v).permute(0, 2, 1, 3).reshape(n, t, nh * hd)
+    for impl, got in outs.items():
+        assert not torch.isnan(got).any(), impl
+        err = (got - ref).abs().max().item()
+        assert err <= 6e-3, (impl, err)
+    assert (outs["wgmma"] - outs["mma"]).abs().max().item() <= 4e-3
+
+
 def test_rmsnorm_swiglu_conv_first(native):
     g = torch.Generator().manual_seed(1)
     m, d, f = 1000, 512, 2048
@@ -127,9 +160,7 @@ def test_gemm_with_fused_swiglu(native, m, k, f):
     x = torch.randn(m, k, generator=g).half()
     w1 = (torch.randn(2 * f, k, generator=g) / k ** 0.5 * 2).half()
     out = torch.full((m, f), float("nan"), dtype=torch.float16, device="cuda")
-    # the largest case also goes through the streaming cta_group::2 pair kernel
-    impl = native.GEMM_TCGEN05_PAIR if (m >= 8192 and (2 * f) % 256 == 0) else native.GEMM_AUTO
-    native.gemm(_dev(x), k, _dev(_interleave_swiglu(w1)), None, out, f, m, 2 * f, k, act=native.ACT_SWIGLU, impl=impl)
+    native.gemm(_dev(x), k, _dev(_interleave_swiglu(w1)), None, out, f, m, 2 * f, k, act=native.ACT_SWIGLU)
     h = (x.float() @ w1.float().t()).half().float()
     y, gate = h.chunk(2, dim=-1)
     ref = (gate * y / (1 + torch.exp(-gate))).half().float()
@@ -168,7 +199,7 @@ def test_sup_width_against_the_reference_fixture(golden_dir):
 
 
 def test_sup_full_depth_matches_same_rounding_oracle():
-    """BASELINE config 3 architecture at full depth (18 layers, d_model 512, 8 heads, k = 5) on two 3996-sample chunks vs
+    """Benchmark config 3 architecture at full depth (18 layers, d_model 512, 8 heads, k = 5) on two 3996-sample chunks vs
     the oracle with fp16 storage rounding.  Budget: scores carry the x5 output scale and reach |x| in [8, 16), where one
     fp16 ulp is 7.8e-3; 18 layers of two half-precision implementations with different accumulation orders stay within
     10 ulp at the worst element, half an ulp on average, and 99 % of all scores within 2 ulp."""
