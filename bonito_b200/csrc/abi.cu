@@ -24,6 +24,13 @@ int lstm_rec_tile_cluster(int hidden);
 int launch_lstm_rec_tile(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
                          int reverse, cudaStream_t stream);
 size_t lstm_rec_tile_workspace_bytes(int N);
+int lstm_rec_wide_ctas(int hidden);
+size_t lstm_rec_wide_workspace_bytes(int N, int hidden);
+size_t lstm_rec_wide_status_offset(int N, int hidden);
+int lstm_rec_wide_max_chunks(int hidden);
+int lstm_rec_wide_resident(int hidden);
+int launch_lstm_rec_wide(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
+                         int reverse, cudaStream_t stream);
 size_t crf_decode_workspace_bytes(int N, int T, int state_len);
 int launch_crf_decode(const __half* scores, int N, int T, int state_len, float blank, float qscale, float qbias,
                       void* workspace, uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream);
@@ -168,6 +175,25 @@ int b200_lstm_rec_tile_fwd(const void* gx, const void* whh, void* y, void* works
     if (t == 0 || n == 0) return 0;
     return launch_lstm_rec_tile((const __half*)gx, (const __half*)whh, (__half*)y, workspace, t, n, hidden, reverse,
                                (cudaStream_t)stream);
+}
+
+int b200_lstm_wide_ctas(int hidden) { return lstm_rec_wide_ctas(hidden); }
+
+int b200_lstm_wide_max_chunks(int hidden) { return lstm_rec_wide_max_chunks(hidden); }
+
+int b200_lstm_wide_resident(int hidden) { return lstm_rec_wide_resident(hidden); }
+
+size_t b200_lstm_rec_wide_workspace_bytes(int n, int hidden) { return lstm_rec_wide_workspace_bytes(n, hidden); }
+
+size_t b200_lstm_rec_wide_status_offset(int n, int hidden) { return lstm_rec_wide_status_offset(n, hidden); }
+
+int b200_lstm_rec_wide_fwd(const void* gx, const void* whh, void* y, void* workspace, int t, int n, int hidden, int reverse,
+                           void* stream) {
+    B200_REQUIRE(gx && whh && y && workspace, "lstm_rec_wide: null pointer argument");
+    B200_REQUIRE(t >= 0 && n >= 0, "lstm_rec_wide: bad sizes t=%d n=%d", t, n);
+    if (t == 0 || n == 0) return 0;
+    return launch_lstm_rec_wide((const __half*)gx, (const __half*)whh, (__half*)y, workspace, t, n, hidden, reverse,
+                                (cudaStream_t)stream);
 }
 
 size_t b200_crf_decode_workspace_bytes(int n, int t, int state_len) {

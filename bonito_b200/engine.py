@@ -1,5 +1,6 @@
 """
-Plan builder + executor for the LSTM-CRF encoder (the `bonito.crf` fast / hac models; LSTM widths 96, 128, 256, 384).
+Plan builder + executor for the LSTM-CRF encoder (the `bonito.crf` fast / hac / LSTM sup models; LSTM widths 96, 128, 256,
+384, 768, 1024).
 
 `compile_lstm_crf(encoder)` walks a `bonito_b200.nn` module tree of the shape the reference's
 configs describe (`bonito/models/configs/dna_r10.4.1@v4.3.toml`,
@@ -23,6 +24,11 @@ be in flight on different streams (`score_batches`, bench.py).
 
 Other widths (`forward_tiled`): the generic `[T][N][4H]` layout and the `mma.sync` recurrent kernel, tiles of 32 chunks
 pipelined on per-tile streams; `B200_LSTM_TILE=0` sends width 384 down this path (8-CTA clusters), `B200_TILE_STREAMS=1` gives the tile-layout path per-tile streams as well (the round-1 schedule).
+
+Widths 768 and 1024 (`forward_wide`: dna_r9.4.1@v3.1, dna_r10.4.1@v4.3): W_hh does not fit the shared memory of one cluster,
+so the recurrence runs on the grid-wide kernel (lstm_rec_wide.cu: H / 8 co-resident CTAs, one cooperative launch per layer);
+activations `[T][N][H]`, gate pre-activations `[T][H/8][N][32]`, layer by layer on the current stream, one buffer set (no
+slots), no int8 input projection.
 """
 
 import torch
@@ -31,6 +37,7 @@ from bonito_b200 import native
 from bonito_b200 import nn as bnn
 
 _ACT_CODES = {None: native.ACT_NONE, "swish": native.ACT_SWISH, "tanh": native.ACT_TANH}
+WIDTHS = (96, 128, 256, 384, 768, 1024)     # LSTM hidden sizes with a native recurrent kernel
 
 
 class UnsupportedModel(NotImplementedError):
@@ -139,8 +146,15 @@ class LstmCrfPlan:
 
         # --- LSTM stack ------------------------------------------------------------------------
         H = self.hidden
+        self.wide = 0                                      # > 0: CTAs of the wide recurrent kernel (H = 768, 1024)
         if native.lstm_cluster_size(H) == 0:
-            raise UnsupportedModel(f"LSTM hidden size {H} has no native kernel")
+            self.wide = native.lstm_wide_ctas(H)
+            if self.wide == 0:
+                raise UnsupportedModel(f"LSTM hidden size {H} has no native kernel (supported: {', '.join(map(str, WIDTHS))})")
+            resident = native.lstm_wide_resident(H, self.device)
+            if resident < self.wide:
+                raise UnsupportedModel(f"the wide LSTM kernel for hidden size {H} needs {self.wide} co-resident CTAs (one per "
+                                       f"SM); this device holds {resident}")
         # H = 384: tile-layout recurrent kernel (64-chunk tiles, 8-CTA clusters, wgmma)
         self.tile = native.lstm_tile_chunks(H)            # 0: only the generic-layout kernel exists for this width
         self.tile_cs = native.lstm_tile_cluster(H)
@@ -197,6 +211,7 @@ class LstmCrfPlan:
         else:
             self.act_l, self.lo, self.hi = crf_act, 0.0, 0.0
         self._bufs = {}
+        self._wide_pending = None   # (event, pinned status words) of the last wide-path forward, checked by the next call
 
     # ------------------------------------------------------------------------------------------
     def frames(self, L):
@@ -549,6 +564,108 @@ class LstmCrfPlan:
             main.wait_event(b["done"][i])
         return out
 
+    # ------------------------------------------------------------------------------------------
+    # wide widths (H = 768, 1024): activations [T][N][H], gate pre-activations [T][G][N][32], one grid-wide recurrent launch
+    # ------------------------------------------------------------------------------------------
+    def _wide_buffers(self, N, L):
+        key = ("wide", N, L)
+        if key not in self._bufs:
+            self._bufs.clear()
+            T = self.frames(L)
+            need = max(self.pad3 + L, (T - 1) * self.s3 + self.k3)
+            Tp = -(-need // self.s3)
+            Lp = Tp * self.s3
+            dev, f16, H = self.device, torch.float16, self.hidden
+            tail = self.k3 * self.c2
+            ws = torch.empty(native.lstm_rec_wide_workspace_bytes(N, H), dtype=torch.uint8, device=dev)
+            off = native.lstm_rec_wide_status_offset(N, H)
+            self._bufs[key] = dict(
+                T=T, Tp=Tp, Lp=Lp,
+                stem=torch.empty(N * Lp * self.c2 + tail, dtype=f16, device=dev),
+                ya=torch.empty(T, N, H, dtype=f16, device=dev),
+                yb=torch.empty(T, N, H, dtype=f16, device=dev),
+                gx=torch.empty(T, self.wide, N, 4 * H // self.wide, dtype=f16, device=dev),
+                ws=ws, ws_status=ws[off:off + 4].view(torch.int32),
+                status=torch.zeros(len(self.lstm), dtype=torch.int32, device=dev),
+            )
+            self._bufs[key]["stem"][-tail:].zero_()
+        return self._bufs[key]
+
+    def _check_wide_status(self):
+        """Raise if a recurrent launch of the previous wide-path forward gave up waiting for its peer CTAs."""
+        pending, self._wide_pending = self._wide_pending, None
+        if pending is not None:
+            done, status = pending
+            done.synchronize()
+            if int(status.max()) != 0:
+                raise native.NativeError(
+                    f"b200_lstm_rec_wide_fwd: the CTAs of the recurrent kernel stopped waiting for each other (status "
+                    f"{status.tolist()} per layer); the scores of the previous batch are invalid")
+
+    def forward_wide(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, return_features=False):
+        """
+        Forward of the wide widths, layer by layer on the current stream: stem -> conv GEMM -> n_lstm x (input GEMM +
+        grid-wide recurrent launch) -> CRF GEMM.  The status words of the recurrent launches are copied to pinned memory at
+        the end and checked at the start of the next call (`_check_wide_status`).  Batches larger than one launch takes
+        (b200_lstm_wide_max_chunks) run as consecutive sub-batches.
+        """
+        self._check_wide_status()
+        if x.dim() == 3:
+            x = x[:, 0, :]
+        x = x.to(device=self.device, dtype=torch.float16).contiguous()
+        N, L = x.shape
+        H, G = self.hidden, self.wide
+        CW = 4 * H // G                     # gx columns per CTA (32)
+        cap = native.lstm_wide_max_chunks(H)
+        if N > cap:
+            if return_features:
+                raise ValueError(f"return_features needs a batch of at most {cap} chunks at hidden size {H}")
+            if out is None:
+                out = torch.empty(N, self.frames(L), self.n_scores, dtype=torch.float16, device=self.device)
+            for n0 in range(0, N, cap):
+                self.forward_wide(x[n0:n0 + cap], out=out[n0:n0 + cap], gemm_impl=gemm_impl, events=events)
+            return out
+        b = self._wide_buffers(N, L)
+        T, Tp, Lp = b["T"], b["Tp"], b["Lp"]
+        feats = {}
+
+        def stage(name):
+            return _Stage(name, events)
+
+        with stage("conv_stem"):
+            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3)
+        if return_features:
+            feats["stem"] = b["stem"][:N * Lp * self.c2].view(N, Lp, self.c2)[:, self.pad3:self.pad3 + L].clone()
+        cur, nxt = b["ya"], b["yb"]
+        with stage("conv_gemm"):
+            native.gemm(b["stem"], self.s3 * self.c2, self.w3, self.b3, cur, H, N * Tp, H, self.k3 * self.c2,
+                        act=self.act3, rows_inner=Tp, valid_inner=T, stride_inner=N, stride_outer=1, impl=gemm_impl)
+        if return_features:
+            feats["conv"] = cur.clone()
+        for i, layer in enumerate(self.lstm):
+            with stage("lstm_in_gemm"):     # rows r = t*N + n -> gx[t][g][n][:], column block g = units [8g, 8g + 8)
+                native.gemm(cur, H, layer["wih"], layer["bias"], b["gx"], CW, T * N, 4 * H, H, rows_inner=N, valid_inner=N,
+                            stride_inner=1, stride_outer=G * N, cb_width=CW, cb_rows=N, impl=gemm_impl)
+            with stage("lstm_rec"):
+                native.lstm_rec_wide(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"], workspace=b["ws"])
+            b["status"][i:i + 1].copy_(b["ws_status"])
+            cur, nxt = nxt, cur
+            if return_features:
+                feats[f"lstm{i}"] = cur.clone()
+
+        if out is None:
+            out = torch.empty(N, T, self.n_scores, dtype=torch.float16, device=self.device)
+        with stage("crf_gemm"):             # rows r = t*N + n -> out[n][t][:]
+            native.gemm(cur, H, self.wl, self.bl, out, self.n_scores, T * N, self.n_scores, H,
+                        act=self.act_l, lo=self.lo, hi=self.hi,
+                        rows_inner=N, valid_inner=N, stride_inner=T, stride_outer=1, impl=gemm_impl)
+        status = torch.empty(len(self.lstm), dtype=torch.int32, pin_memory=True)
+        status.copy_(b["status"], non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        self._wide_pending = (done, status)
+        return (out, feats) if return_features else out
+
     def forward(self, x, out=None, gemm_impl=native.GEMM_AUTO, return_features=False, events=None, tiled=None,
                 decode=None, slot=0):
         with torch.cuda.device(self.device):    # streams / events / launches belong to the plan's device, whatever is current
@@ -574,6 +691,8 @@ class LstmCrfPlan:
                                       streams=tiled, slot=slot)
         if slot != 0:
             raise NotImplementedError("several batches in flight (slot != 0) need the tile-layout path (hidden size 384)")
+        if self.wide:
+            return self.forward_wide(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features)
         if tiled is None:
             tiled = (not return_features) and x.shape[0] > self.TILE
         if tiled:

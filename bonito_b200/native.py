@@ -58,6 +58,12 @@ SIGNATURES = {
     "b200_lstm_tile_cluster": (c_int, [c_int]),
     "b200_lstm_rec_tile_workspace_bytes": (c_size_t, [c_int]),
     "b200_lstm_rec_tile_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "b200_lstm_wide_ctas": (c_int, [c_int]),
+    "b200_lstm_wide_max_chunks": (c_int, [c_int]),
+    "b200_lstm_wide_resident": (c_int, [c_int]),
+    "b200_lstm_rec_wide_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b200_lstm_rec_wide_status_offset": (c_size_t, [c_int, c_int]),
+    "b200_lstm_rec_wide_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "b200_crf_decode_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "b200_quantize_i8": (c_int, [c_void_p, c_void_p, c_longlong, c_float, c_void_p]),
     "b200_stream_create": (c_int, [c_void_p]),
@@ -235,6 +241,46 @@ def lstm_rec_tile(gx, whh, y, t, n, hidden, reverse, stream=None, workspace=None
         rc = lib.b200_lstm_rec_tile_fwd(_ptr(gx), _ptr(_f16(whh, "whh")), _ptr(y), _ptr(workspace), t, n, hidden,
                                         int(bool(reverse)), _stream(stream))
     _check(rc, "b200_lstm_rec_tile_fwd")
+    return y
+
+
+def lstm_wide_ctas(hidden):
+    """CTAs of the wide recurrent kernel (hidden / 8; 0: this hidden size has no wide kernel)."""
+    return load().b200_lstm_wide_ctas(hidden)
+
+
+def lstm_wide_max_chunks(hidden):
+    return load().b200_lstm_wide_max_chunks(hidden)
+
+
+def lstm_wide_resident(hidden, device=None):
+    """CTAs of the wide kernel that fit on the device at once (the grid needs lstm_wide_ctas(hidden) of them)."""
+    lib = require()
+    with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+        rc = lib.b200_lstm_wide_resident(hidden)
+    if rc < 0:
+        _check(rc, "b200_lstm_wide_resident")
+    return rc
+
+
+def lstm_rec_wide_workspace_bytes(n, hidden):
+    return load().b200_lstm_rec_wide_workspace_bytes(n, hidden)
+
+
+def lstm_rec_wide_status_offset(n, hidden):
+    return load().b200_lstm_rec_wide_status_offset(n, hidden)
+
+
+def lstm_rec_wide(gx, whh, y, t, n, hidden, reverse, stream=None, workspace=None):
+    """gx [T][G][n][32], y [T][n][H] (see b200_lstm_rec_wide_fwd).  `workspace`: uint8 tensor of
+    lstm_rec_wide_workspace_bytes(n, hidden) bytes (allocated here when omitted); its status word is not checked here."""
+    lib = require()
+    if workspace is None:
+        workspace = torch.empty(lstm_rec_wide_workspace_bytes(n, hidden), dtype=torch.uint8, device=y.device)
+    with torch.cuda.device(y.device):
+        rc = lib.b200_lstm_rec_wide_fwd(_ptr(gx), _ptr(_f16(whh, "whh")), _ptr(y), _ptr(workspace), t, n, hidden,
+                                        int(bool(reverse)), _stream(stream))
+    _check(rc, "b200_lstm_rec_wide_fwd")
     return y
 
 

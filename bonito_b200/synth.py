@@ -18,6 +18,7 @@ SHAPES = {
     "fast": (96, 3),
     "hac": (384, 4),
     "tiny": (96, 3),
+    "sup_lstm": (1024, 5),     # dna_r10.4.1@v4.3, the LSTM sup model: the same layer stack at width 1024
 }
 
 
@@ -31,8 +32,38 @@ def model_spec(name="hac", n_lstm=5, stride=6, winlen=19):
     )
 
 
+def old_style_spec(n_lstm=5):
+    """dna_r9.4.1@v3.1: the old-style `[encoder]` (built by rnn_encoder, bonito/crf/model.py:150-162): 1 -> 4 -> 16 stem,
+    conv3 k19 stride 5 swish into width 768, LSTMs reversed (n_lstm - i) % 2, LinearCRFEncoder with bias, tanh, scale 5."""
+    return dict(
+        name="r9_v3.1", hidden=768, state_len=5, n_lstm=n_lstm,
+        convs=[(1, 4, 5, 1, 2, "swish"), (4, 16, 5, 1, 2, "swish"), (16, 768, 19, 5, 9, "swish")],
+        reverse=[bool((n_lstm - i) % 2) for i in range(n_lstm)],
+        blank_score=2.0, clamp=None, stride=5, crf_activation="tanh", crf_scale=5.0, crf_bias=True, old_style=True,
+    )
+
+
+def old_style_config(spec, batchsize=32, chunksize=4000, overlap=500):
+    """TOML-equivalent dict of an old-style config (the keys of dna_r9.4.1@v3.1.toml)."""
+    enc = dict(stride=spec["convs"][2][3], winlen=spec["convs"][2][2], scale=spec["crf_scale"], features=spec["hidden"],
+               rnn_type="lstm", activation=spec["convs"][2][5], blank_score=spec["blank_score"])
+    if spec["n_lstm"] != 5:
+        enc["num_layers"] = spec["n_lstm"]
+    return {
+        "model": {"package": "bonito.crf"},
+        "labels": {"labels": ["N", "A", "C", "G", "T"]},
+        "input": {"features": 1},
+        "qscore": {"bias": 0.0, "scale": 1.0},
+        "encoder": enc,
+        "global_norm": {"state_len": spec["state_len"]},
+        "basecaller": {"batchsize": batchsize, "chunksize": chunksize, "overlap": overlap},
+    }
+
+
 def model_config(spec, batchnorm=False, batchsize=32, chunksize=3996, overlap=492):
-    """TOML-equivalent dict for `Model(config)` (layout of dna_r10.4.1@v4.3.toml)."""
+    """TOML-equivalent dict for `Model(config)` (layout of dna_r10.4.1@v4.3.toml; `old_style_config` for old_style specs)."""
+    if spec.get("old_style"):
+        return old_style_config(spec, batchsize=batchsize, chunksize=chunksize, overlap=overlap)
     sub = []
     for cin, cout, k, s, p, act in spec["convs"]:
         layer = dict(type="convolution", insize=cin, size=cout, bias=True, winlen=k, stride=s, padding=p, activation=act)
@@ -65,15 +96,16 @@ def model_config(spec, batchnorm=False, batchsize=32, chunksize=3996, overlap=49
     }
 
 
-def _orthogonal_blocks(rows, cols, block, gen, gain):
+def _orthogonal_blocks(rows, cols, block, gen, gain, f64=False):
     w = torch.empty(rows, cols)
     for r in range(0, rows, block):
-        q, _ = torch.linalg.qr(torch.randn(max(block, cols), max(block, cols), generator=gen))
-        w[r:r + block] = q[:block, :cols]
+        g = torch.randn(max(block, cols), max(block, cols), generator=gen)
+        q, _ = torch.linalg.qr(g.double() if f64 else g)
+        w[r:r + block] = q[:block, :cols].float()
     return w * gain
 
 
-def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp16_values=True):
+def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp16_values=True, qr_f64=False):
     """
     Seeded, non-degenerate weights (oracle naming).  The reference's own init (orthogonal LSTM blocks,
     0.5*truncated-normal input bias, zero state bias: bonito/nn.py:362-390) with gains chosen so that
@@ -81,6 +113,8 @@ def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp1
     recurrence stays well conditioned (an LSTM gain of 3 makes the stack chaotic: a 1e-3 input perturbation grows to
     O(1) score differences, so no two half-precision implementations could agree; at 1.5 it shrinks).
     With `fp16_values` every tensor is rounded to fp16 (what `model.half()` feeds every implementation).
+    `qr_f64=True` factorises the same Gaussian draws in float64: the fp16-rounded weights are then the same on every
+    CPU (the float32 QR may round differently elsewhere), for fixtures that store a digest instead of the weights.
     """
     gen = torch.Generator().manual_seed(seed)
     H = spec["hidden"]
@@ -90,12 +124,14 @@ def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp1
         w[f"conv{i}.weight"] = torch.randn(cout, cin, k, generator=gen) * (conv_gain / fan_in ** 0.5)
         w[f"conv{i}.bias"] = torch.randn(cout, generator=gen) * 0.1
     for i in range(spec["n_lstm"]):
-        w[f"lstm{i}.w_ih"] = _orthogonal_blocks(4 * H, H, H, gen, lstm_gain)
-        w[f"lstm{i}.w_hh"] = _orthogonal_blocks(4 * H, H, H, gen, lstm_gain)
+        w[f"lstm{i}.w_ih"] = _orthogonal_blocks(4 * H, H, H, gen, lstm_gain, qr_f64)
+        w[f"lstm{i}.w_hh"] = _orthogonal_blocks(4 * H, H, H, gen, lstm_gain, qr_f64)
         w[f"lstm{i}.b_ih"] = 0.5 * torch.randn(4 * H, generator=gen).clamp(-2, 2)
         w[f"lstm{i}.b_hh"] = torch.zeros(4 * H)
     C = 4 ** (spec["state_len"] + 1)
     w["crf.weight"] = torch.randn(C, H, generator=gen) * (head_gain / H ** 0.5)
+    if spec.get("crf_bias"):                 # old-style heads (LinearCRFEncoder default bias=True)
+        w["crf.bias"] = torch.randn(C, generator=gen) * 0.1
     if fp16_values:
         w = {k: v.half().float() for k, v in w.items()}
     return w
@@ -115,6 +151,8 @@ def state_dict_from_weights(spec, weights, prefix="encoder."):
         sd[f"{prefix}{base + i}.rnn.bias_ih_l0"] = weights[f"lstm{i}.b_ih"]
         sd[f"{prefix}{base + i}.rnn.bias_hh_l0"] = weights[f"lstm{i}.b_hh"]
     sd[f"{prefix}{base + spec['n_lstm']}.linear.weight"] = weights["crf.weight"]
+    if "crf.bias" in weights:
+        sd[f"{prefix}{base + spec['n_lstm']}.linear.bias"] = weights["crf.bias"]
     return sd
 
 

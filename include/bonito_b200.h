@@ -127,6 +127,34 @@ int b200_lstm_rec_tile_fwd(const void* gx, const void* whh, void* y, void* works
                            int reverse, void* stream);
 
 /*
+ * Wide recurrent kernel, hidden = 768 and 1024 (dna_r9.4.1@v3.1, dna_r10.4.1@v4.3): W_hh is spread over G = hidden / 8 CTAs
+ * (8 units = 32 gate columns each, slice resident in shared memory), one cooperative launch per layer, wgmma on 64-chunk
+ * tiles, h exchanged through L2 with a grid-wide barrier every step.  b200_lstm_cluster_size() keeps returning 0 for these
+ * widths: it describes the generic kernel.
+ *   b200_lstm_wide_ctas(hidden)        G (96 / 128), 0 = this hidden size has no wide kernel
+ *   b200_lstm_wide_max_chunks(hidden)  largest n one launch accepts (2560)
+ *   b200_lstm_wide_resident(hidden)    CTAs of the kernel that can be resident at once on the current device (negative on
+ *                                      error); the grid only launches if this is >= G
+ *   gx  [T][G][n][32]   columns of CTA g: [unit - 8g][gate i,f,g,o]  (b200_gemm_fwd_ex with W_ih / bias in [unit][gate]
+ *                       row order, rows (t, chunk): rows_inner = n, stride_inner = 1, stride_outer = G*n, cb_width = 32,
+ *                       cb_rows = n, ldc = 32)
+ *   whh [4H][H]         as for b200_lstm_rec_fwd
+ *   y   [T][n][H]       h_t in natural unit order
+ *   workspace           b200_lstm_rec_wide_workspace_bytes(n, hidden) bytes: h exchange buffer, barrier counter and status
+ *                       word (reset on the stream by every launch); launches that may run concurrently need distinct
+ *                       workspaces
+ * Status: the uint32 at byte offset b200_lstm_rec_wide_status_offset(n, hidden) of the workspace is 0 after a launch that
+ * completed, non-zero if the CTAs stopped waiting for each other (a bounded wait expired) and y is not valid.
+ */
+int b200_lstm_wide_ctas(int hidden);
+int b200_lstm_wide_max_chunks(int hidden);
+int b200_lstm_wide_resident(int hidden);
+size_t b200_lstm_rec_wide_workspace_bytes(int n, int hidden);
+size_t b200_lstm_rec_wide_status_offset(int n, int hidden);
+int b200_lstm_rec_wide_fwd(const void* gx, const void* whh, void* y, void* workspace, int t, int n, int hidden, int reverse,
+                           void* stream);
+
+/*
  * ---- transformer (sup) path: bonito/transformer/model.py ----
  *
  * First convolution of a conv stack: x[N][L] -> Conv1d(1->c, k, pad k/2) + act, channels-last with zero halo:
