@@ -135,8 +135,7 @@ def score_batches(model, batches, depth=2, beam_width=32, beam_cut=100.0, scale=
                 if slot.dev_out is None:
                     slot.dev_out = torch.empty(3, n, t, dtype=torch.uint8, device=device)
                     slot.pinned_out = torch.empty(3, n, t, dtype=torch.uint8, pin_memory=True)
-                state_len = int(round(np.log(c) / np.log(4))) - 1
-                _decoder(scores, state_len, blank_score=blank_score, qscale=scale, qbias=offset, out=slot.dev_out,
+                _decoder(scores, model.seqdist.state_len, blank_score=blank_score, qscale=scale, qbias=offset, out=slot.dev_out,
                          slot=slot.index)
                 slot.pinned_out.copy_(slot.dev_out, non_blocking=True)
                 slot.done.record(main)
@@ -186,9 +185,12 @@ def _supports_slots(model, device):
 
 
 def _revcomp_native(model, scores, blank_score):
-    """[N,T,C] (no blanks) -> reverse-complemented [N,T,C] through the reference's [T,N,C+blanks] definition."""
+    """[N,T,C] -> reverse-complemented [N,T,C] through the reference's [T,N,C+blanks] definition.  Fixed-blank scores (no
+    blank column) are padded with `blank_score` and unpadded again; learned-blank scores already are that layout."""
     n, t, c = scores.shape
     nb = model.seqdist.n_base
+    if c == model.seqdist.n_score():
+        return model.seqdist.reverse_complement(scores.permute(1, 0, 2)).permute(1, 0, 2).contiguous()
     full = torch.nn.functional.pad(scores.permute(1, 0, 2).reshape(t, n, c // nb, nb), (1, 0), value=blank_score)
     rc = model.seqdist.reverse_complement(full.reshape(t, n, -1)).reshape(t, n, c // nb, nb + 1)
     return rc[..., 1:].reshape(t, n, c).permute(1, 0, 2).contiguous()

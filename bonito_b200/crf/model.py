@@ -165,22 +165,27 @@ class SeqdistModel(Module):
     # -- decode ------------------------------------------------------------------------------------
     def decode_batch(self, x):
         """
-        x: scores.  Native layout [N, T, C] (no blanks) on CUDA -> list of N strings, via the sm_90a
-        posterior-Viterbi kernel (same maths as the reference's decode_batch, bonito/crf/model.py:196-199).
+        x: scores.  Native layout [N, T, C] on CUDA (no blank column, or the [state][stay, m0..m3] layout of a head with
+        learned blank scores) -> list of N strings, via the sm_90a posterior-Viterbi kernel (same maths as the reference's decode_batch, bonito/crf/model.py:196-199).
         """
         from bonito_b200.decode import beam_search, to_str
         if not x.is_cuda:
             raise NotImplementedError("decode_batch runs on the native CUDA decoder only")
-        seq, _, _ = beam_search(x.contiguous(), blank_score=self._blank_score())
+        blank = self._blank_score()
+        if blank is None:        # learned blank scores: the stay scores are columns of x, there is no fixed one to pass
+            seq, _, _ = beam_search(x.contiguous())
+        else:
+            seq, _, _ = beam_search(x.contiguous(), blank_score=blank)
         return [to_str(row) for row in seq]
 
     def decode(self, x):
         return self.decode_batch(x.unsqueeze(0))[0]
 
     def _blank_score(self):
+        """The head's fixed blank score; None when the head learns its blank scores (blank_score=None)."""
         for m in self.encoder.modules():
-            if isinstance(m, LinearCRFEncoder) and m.blank_score is not None:
-                return float(m.blank_score)
+            if isinstance(m, LinearCRFEncoder):
+                return None if m.blank_score is None else float(m.blank_score)
         return 2.0
 
     def to_dict(self, include_weights=False):

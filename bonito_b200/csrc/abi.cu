@@ -8,7 +8,7 @@
 
 int launch_conv_stem(const __half* x, int N, int L, int C1, int K1, const __half* w1, const __half* b1, int act1,
                      int C2, int K2, const __half* w2, const __half* b2, int act2, __half* out, int Lp, int padl,
-                     cudaStream_t stream);
+                     float lo1, float hi1, float lo2, float hi2, cudaStream_t stream);
 int lstm_rec_cluster_size(int H);
 int launch_lstm_rec(const __half* gx, const __half* whh, __half* y, int T, int N, int H, int reverse,
                     cudaStream_t stream);
@@ -34,6 +34,8 @@ int launch_lstm_rec_wide(const __half* gx, const __half* whh, __half* y, void* w
 size_t crf_decode_workspace_bytes(int N, int T, int state_len);
 int launch_crf_decode(const __half* scores, int N, int T, int state_len, float blank, float qscale, float qbias,
                       void* workspace, uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream);
+int launch_crf_decode_lb(const __half* scores, int N, int T, int state_len, float qscale, float qbias, void* workspace,
+                         uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream);
 
 // one message buffer per host thread: the reference drives this path from background threads (bonito/multiprocessing.py:118-122),
 // so a failing call must read back its own message, not another thread's
@@ -64,11 +66,18 @@ const char* b200_last_error(void) { return g_err; }
 int b200_conv_stem_fwd(const void* x, int n, int l, int c1, int k1, const void* w1, const void* b1, int act1,
                        int c2, int k2, const void* w2, const void* b2, int act2, void* out, int lp, int padl,
                        void* stream) {
+    return b200_conv_stem_fwd_ex(x, n, l, c1, k1, w1, b1, act1, 0.f, 0.f, c2, k2, w2, b2, act2, 0.f, 0.f, out, lp, padl,
+                                 stream);
+}
+
+int b200_conv_stem_fwd_ex(const void* x, int n, int l, int c1, int k1, const void* w1, const void* b1, int act1, float lo1,
+                          float hi1, int c2, int k2, const void* w2, const void* b2, int act2, float lo2, float hi2, void* out,
+                          int lp, int padl, void* stream) {
     B200_REQUIRE(x && w1 && w2 && out, "conv_stem: null pointer argument");
     B200_REQUIRE(n >= 0 && l > 0 && lp >= padl + l, "conv_stem: bad sizes n=%d l=%d lp=%d padl=%d", n, l, lp, padl);
     if (n == 0) return 0;
     return launch_conv_stem((const __half*)x, n, l, c1, k1, (const __half*)w1, (const __half*)b1, act1, c2, k2,
-                            (const __half*)w2, (const __half*)b2, act2, (__half*)out, lp, padl,
+                            (const __half*)w2, (const __half*)b2, act2, (__half*)out, lp, padl, lo1, hi1, lo2, hi2,
                             (cudaStream_t)stream);
 }
 
@@ -207,6 +216,16 @@ int b200_crf_decode(const void* scores, int n, int t, int state_len, float blank
     B200_REQUIRE(scores && workspace && moves && sequence && qstring, "crf_decode: null pointer argument");
     return launch_crf_decode((const __half*)scores, n, t, state_len, blank_score, qscale, qbias, workspace,
                              (uint8_t*)moves, (uint8_t*)sequence, (uint8_t*)qstring, (cudaStream_t)stream);
+}
+
+int b200_crf_decode_lb(const void* scores, int n, int t, int state_len, float qscale, float qbias, void* workspace, void* moves,
+                       void* sequence, void* qstring, void* stream) {
+    B200_REQUIRE(n >= 0 && t >= 0, "crf_decode_lb: bad sizes n=%d t=%d", n, t);
+    if (n == 0 || t == 0) return 0;
+    B200_REQUIRE(scores && workspace && moves && sequence && qstring, "crf_decode_lb: null pointer argument");
+    B200_REQUIRE(((uintptr_t)scores & 15) == 0, "crf_decode_lb: scores must be 16-byte aligned");
+    return launch_crf_decode_lb((const __half*)scores, n, t, state_len, qscale, qbias, workspace, (uint8_t*)moves,
+                                (uint8_t*)sequence, (uint8_t*)qstring, (cudaStream_t)stream);
 }
 
 int b200_chunk_count(long long length, int chunksize, int overlap) {

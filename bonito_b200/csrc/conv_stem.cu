@@ -17,7 +17,7 @@ template <int C1, int K1, int C2, int K2>
 __global__ void __launch_bounds__(TL)
 conv_stem_kernel(const __half* __restrict__ x, int L, const __half* __restrict__ w1, const __half* __restrict__ b1,
                  int act1, const __half* __restrict__ w2, const __half* __restrict__ b2, int act2,
-                 __half* __restrict__ out, int Lp, int padl) {
+                 __half* __restrict__ out, int Lp, int padl, float lo1, float hi1, float lo2, float hi2) {
     constexpr int P1 = K1 / 2, P2 = K2 / 2;
     constexpr int NA1 = TL + K2 - 1;        // conv1 outputs needed by this tile
     constexpr int NX = NA1 + K1 - 1;        // input samples needed
@@ -61,7 +61,7 @@ conv_stem_kernel(const __half* __restrict__ x, int L, const __half* __restrict__
             float acc = b1s[c];
 #pragma unroll
             for (int k = 0; k < K1; ++k) acc = fmaf(w1s[k][c], xv[k], acc);
-            a1s[c][i] = in ? apply_act_f16(acc, act1, 0.f, 0.f) : 0.f;
+            a1s[c][i] = in ? apply_act_f16(acc, act1, lo1, hi1) : 0.f;
         }
     }
     __syncthreads();
@@ -99,8 +99,8 @@ conv_stem_kernel(const __half* __restrict__ x, int L, const __half* __restrict__
         __half2 h[4];
 #pragma unroll
         for (int q = 0; q < 4; ++q)
-            h[q] = __floats2half2_rn(apply_act_f16(acc[c + 2 * q], act2, 0.f, 0.f),
-                                     apply_act_f16(acc[c + 2 * q + 1], act2, 0.f, 0.f));
+            h[q] = __floats2half2_rn(apply_act_f16(acc[c + 2 * q], act2, lo2, hi2),
+                                     apply_act_f16(acc[c + 2 * q + 1], act2, lo2, hi2));
         *reinterpret_cast<uint4*>(dst + c) = *reinterpret_cast<uint4*>(h);
     }
 }
@@ -118,7 +118,7 @@ constexpr int TC_THREADS = TL + 32;   // eight GEMM warps + one more so that the
 __global__ void __launch_bounds__(TC_THREADS, 2)
 conv_stem_tc_kernel(const __half* __restrict__ x, int L, const __half* __restrict__ w1, const __half* __restrict__ b1,
                     int act1, const __half* __restrict__ w2, const __half* __restrict__ b2, int act2,
-                    __half* __restrict__ out, int Lp, int padl) {
+                    __half* __restrict__ out, int Lp, int padl, float lo1, float hi1, float lo2, float hi2) {
     constexpr int C1 = 16, K1 = 5, C2 = 16, K2 = 5, P1 = K1 / 2, P2 = K2 / 2;
     constexpr int NA1 = TL + K2 - 1, NX = NA1 + K1 - 1;
     __shared__ float xs[NX];
@@ -158,7 +158,7 @@ conv_stem_tc_kernel(const __half* __restrict__ x, int L, const __half* __restric
                 acc0 = fmaf(w1s[k][c], xv[k], acc0);
                 acc1 = fmaf(w1s[k][c + 1], xv[k], acc1);
             }
-            h[c / 2] = in ? __floats2half2_rn(apply_act_f16(acc0, act1, 0.f, 0.f), apply_act_f16(acc1, act1, 0.f, 0.f))
+            h[c / 2] = in ? __floats2half2_rn(apply_act_f16(acc0, act1, lo1, hi1), apply_act_f16(acc1, act1, lo1, hi1))
                           : __floats2half2_rn(0.f, 0.f);
         }
         *reinterpret_cast<uint4*>(&a1h[i][0]) = *reinterpret_cast<const uint4*>(&h[0]);
@@ -207,8 +207,8 @@ conv_stem_tc_kernel(const __half* __restrict__ x, int L, const __half* __restric
         }
 #pragma unroll
         for (int nt = 0; nt < 2; ++nt) {
-            const __half2 lo = __floats2half2_rn(apply_act_f16(acc[nt][0], act2, 0.f, 0.f), apply_act_f16(acc[nt][1], act2, 0.f, 0.f));
-            const __half2 hi = __floats2half2_rn(apply_act_f16(acc[nt][2], act2, 0.f, 0.f), apply_act_f16(acc[nt][3], act2, 0.f, 0.f));
+            const __half2 lo = __floats2half2_rn(apply_act_f16(acc[nt][0], act2, lo2, hi2), apply_act_f16(acc[nt][1], act2, lo2, hi2));
+            const __half2 hi = __floats2half2_rn(apply_act_f16(acc[nt][2], act2, lo2, hi2), apply_act_f16(acc[nt][3], act2, lo2, hi2));
             *reinterpret_cast<__half2*>(&stage[warp][mt * 16 + g][nt * 8 + 2 * q]) = lo;
             *reinterpret_cast<__half2*>(&stage[warp][mt * 16 + g + 8][nt * 8 + 2 * q]) = hi;
         }
@@ -232,18 +232,18 @@ conv_stem_tc_kernel(const __half* __restrict__ x, int L, const __half* __restric
 
 int launch_conv_stem(const __half* x, int N, int L, int C1, int K1, const __half* w1, const __half* b1, int act1,
                      int C2, int K2, const __half* w2, const __half* b2, int act2, __half* out, int Lp, int padl,
-                     cudaStream_t stream) {
+                     float lo1, float hi1, float lo2, float hi2, cudaStream_t stream) {
     dim3 grid((Lp + TL - 1) / TL, N);
     const char* impl = getenv("B200_STEM_IMPL");   // "fma": the CUDA-core kernel for every shape
     if (C1 == 16 && K1 == 5 && C2 == 16 && K2 == 5 && !(impl && impl[0] == 'f')) {
-        conv_stem_tc_kernel<<<grid, TC_THREADS, 0, stream>>>(x, L, w1, b1, act1, w2, b2, act2, out, Lp, padl);
+        conv_stem_tc_kernel<<<grid, TC_THREADS, 0, stream>>>(x, L, w1, b1, act1, w2, b2, act2, out, Lp, padl, lo1, hi1, lo2, hi2);
         B200_CHECK_CUDA(cudaGetLastError());
         return 0;
     }
 #define STEM_CASE(c1, k1, c2, k2)                                                                         \
     if (C1 == c1 && K1 == k1 && C2 == c2 && K2 == k2) {                                                   \
         conv_stem_kernel<c1, k1, c2, k2><<<grid, TL, 0, stream>>>(x, L, w1, b1, act1, w2, b2, act2, out,  \
-                                                                  Lp, padl);                              \
+                                                                  Lp, padl, lo1, hi1, lo2, hi2);          \
         B200_CHECK_CUDA(cudaGetLastError());                                                              \
         return 0;                                                                                         \
     }

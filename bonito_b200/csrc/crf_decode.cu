@@ -17,6 +17,15 @@
 //   pass 3: trace-back through the back-pointers (staged through shared memory in blocks)
 // Tie-breaks (the reference's are whatever argmax over koi's Max-semiring gradient gives):
 // lowest in-edge index, lowest final state.
+//
+// Learned blank scores (LB = true, b200_crf_decode_lb): heads without a fixed blank_score emit the stay score of every state at
+// every frame, [N][T][S*5] in the CTC_CRF layout [state][stay, move 0..3].  Rows of 10*S bytes do not split into one aligned
+// 8-byte piece per thread, so each score row is copied whole into the shared-memory ring with cooperative 16-byte cp.async
+// copies (5S/8 threads, one piece each) and every thread reads its five values from there.  A thread now reads what other
+// threads copied, so a row must be complete and published by a barrier before its step: the rings run one step further
+// ahead (each step waits for the row after next) and the per-step barrier that is already there publishes it.  Every other
+// line of the three passes is the fixed-blank code, which these rows also keep bit-identical when the stay column is the
+// fixed score.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -38,7 +47,7 @@ __device__ __forceinline__ float lse2_5(float a, float b, float c, float d, floa
     return m + lg2_approx(s);
 }
 
-template <int S>
+template <int S, bool LB>
 struct DecodeSmem {
     static constexpr int NW = (S + 31) / 32;
     static constexpr int TB = 16384 / S;                 // back-pointer rows per trace-back block
@@ -48,8 +57,9 @@ struct DecodeSmem {
     static constexpr size_t kPart = kUnion + kUnionBytes;              // float [2][NW][4]
     static constexpr size_t kKt = kPart + 2 * NW * 4 * sizeof(float);  // float [2]: per-step posterior normaliser
     static constexpr int PF = 4;                                       // prefetch depth (steps) of the cp.async rings
-    static constexpr size_t kScRing = kKt + 16;                        // uint2 [PF][S]: score rows in flight
-    static constexpr size_t kBetaRing = kScRing + PF * S * sizeof(uint2);   // float [PF][S]: beta' rows in flight (pass 2)
+    static constexpr size_t kScRow = LB ? 5 * S * sizeof(__half) : S * sizeof(uint2);   // bytes per score row
+    static constexpr size_t kScRing = kKt + 16;                        // [PF] score rows in flight: uint2 [S] | half [S][5]
+    static constexpr size_t kBetaRing = kScRing + PF * kScRow;         // float [PF][S]: beta' rows in flight (pass 2)
     static constexpr size_t kRed = kBetaRing + PF * S * sizeof(float);
     static constexpr size_t kRedI = kRed + NW * sizeof(float);
     static constexpr size_t kOut = kRedI + NW * sizeof(int) + 16;      // u8 [3][T]
@@ -74,13 +84,13 @@ __device__ __forceinline__ void cp_async_4(void* smem_dst, const void* gmem_src)
 // in the natural-log domain: 195 + 86 SASS instructions per forward / backward state-step, a third of them the FMUL /
 // FSETP range handling around each MUFU; this one needs ~105 + ~55.)  The step loops are unrolled by two so that every
 // buffer that flips with the step parity is a compile-time address.
-template <int S>
+template <int S, bool LB>
 __global__ void __launch_bounds__(S)
 crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float qscale, float qbias,
                   float* __restrict__ ws_beta, double* __restrict__ ws_bsum, uint8_t* __restrict__ ws_bp,
                   float* __restrict__ ws_pm, uint8_t* __restrict__ moves, uint8_t* __restrict__ seq,
                   uint8_t* __restrict__ qual) {
-    using L = DecodeSmem<S>;
+    using L = DecodeSmem<S, LB>;
     constexpr int Q = S / 4, NW = L::NW, TB = L::TB;
     extern __shared__ __align__(16) unsigned char sm[];
     float (*buf)[S] = reinterpret_cast<float (*)[S]>(sm + L::kAv);            // pass 1: beta'
@@ -91,6 +101,7 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
     float* kt_sh = reinterpret_cast<float*>(sm + L::kKt);
     constexpr int PF = L::PF;
     uint2 (*sc_ring)[S] = reinterpret_cast<uint2 (*)[S]>(sm + L::kScRing);
+    unsigned char* sc_ring_lb = sm + L::kScRing;                             // LB: half [PF][S][5]
     float (*beta_ring)[S] = reinterpret_cast<float (*)[S]>(sm + L::kBetaRing);
     float* red = reinterpret_cast<float*>(sm + L::kRed);
     int* red_i = reinterpret_cast<int*>(sm + L::kRedI);
@@ -101,6 +112,18 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
     const int s = threadIdx.x;
     const int lane = s & 31, warp = s >> 5;
     const uint2* sc = reinterpret_cast<const uint2*>(scores + (size_t)n * T * S * 4) + s;  // row stride S
+    const unsigned char* sc_lb = reinterpret_cast<const unsigned char*>(scores + (size_t)n * T * S * 5);  // LB: rows of kScRow B
+    // score row r -> ring slot r % PF: fixed blank, this thread's 8 bytes; learned blank, the whole row in 16-byte pieces
+    auto fetch_row = [&](int r) {
+        if constexpr (LB) {
+            if (s < (int)(L::kScRow / 16))
+                cp_async_16(sc_ring_lb + (r & (PF - 1)) * L::kScRow + s * 16, sc_lb + (size_t)r * L::kScRow + s * 16, true);
+        } else {
+            cp_async_8(&sc_ring[r & (PF - 1)][s], sc + (size_t)r * S);
+        }
+    };
+    // LB: the five scores of state s in ring slot `slot`
+    auto lb_row = [&](int slot) { return reinterpret_cast<const __half*>(sc_ring_lb + slot * L::kScRow) + 5 * s; };
     float* beta = ws_beta + (size_t)n * (T + 1) * S;
     double* bsum = ws_bsum + (size_t)n * (T + 1);
     uint8_t* bp = ws_bp + (size_t)n * T * S;
@@ -122,12 +145,24 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
             dst[0 * S + s] = m01.x * LOG2E; dst[1 * S + s] = m01.y * LOG2E;
             dst[2 * S + s] = m23.x * LOG2E; dst[3 * S + s] = m23.y * LOG2E;
         };
-        scatter(msh[0], sc[(size_t)(T - 1) * S]);
+        // LB: the moves of state s from its five scores [stay, m0..m3]; returns the stay score (log2 units)
+        auto scatter_lb = [&](float* dst, const __half* e) {
+            dst[0 * S + s] = __half2float(e[1]) * LOG2E; dst[1 * S + s] = __half2float(e[2]) * LOG2E;
+            dst[2 * S + s] = __half2float(e[3]) * LOG2E; dst[3 * S + s] = __half2float(e[4]) * LOG2E;
+            return __half2float(e[0]) * LOG2E;
+        };
+        float stay_cur = blank2;                                   // LB: stay score of state s at the current step
+        if constexpr (LB) {
+            stay_cur = scatter_lb(msh[0], reinterpret_cast<const __half*>(sc_lb + (size_t)(T - 1) * L::kScRow) + 5 * s);
+        } else {
+            scatter(msh[0], sc[(size_t)(T - 1) * S]);
+        }
         // score rows T-2, T-3, ... travel through the ring: row r lives in slot r % PF; PF-1 groups are kept in flight
         for (int r = T - 2; r > T - 2 - (PF - 1); --r) {
-            if (r >= 0) cp_async_8(&sc_ring[r & (PF - 1)][s], sc + (size_t)r * S);
+            if (r >= 0) fetch_row(r);
             cp_async_commit();
         }
+        if constexpr (LB) cp_async_wait<PF - 2>();                 // row T-2, published by the barrier below
         float* beta_p = beta + (size_t)(T - 1) * S + s;
         double* bsum_p = bsum + (T - 1);
         double acc_shift = 0.0;
@@ -135,16 +170,24 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
         auto bwd = [&](int t, auto cur_c) {
             constexpr int CUR = decltype(cur_c)::value;
             {   // next row into the ring (row t-PF; its slot held row t, scattered in the previous step), then wait for row t-1
+                // (LB: for row t-2, which the barrier at the end of this step publishes for the next one)
                 const int r = t - PF;
-                if (r >= 0) cp_async_8(&sc_ring[r & (PF - 1)][s], sc + (size_t)r * S);
+                if (r >= 0) fetch_row(r);
                 cp_async_commit();
-                cp_async_wait<PF - 1>();
+                if constexpr (LB) cp_async_wait<PF - 2>();
+                else cp_async_wait<PF - 1>();
             }
-            if (t > 0) scatter(msh[CUR ^ 1], sc_ring[(t - 1) & (PF - 1)][s]);
+            [[maybe_unused]] float stay_next = 0.f;
+            if constexpr (LB) {
+                if (t > 0) stay_next = scatter_lb(msh[CUR ^ 1], lb_row((t - 1) & (PF - 1)));
+            } else {
+                if (t > 0) scatter(msh[CUR ^ 1], sc_ring[(t - 1) & (PF - 1)][s]);
+            }
             const float b0 = buf[CUR][0];
             const float4 mv = *reinterpret_cast<const float4*>(&msh[CUR][4 * s]);
             const float4 bs = *reinterpret_cast<const float4*>(&buf[CUR][4 * (s % Q)]);
-            const float v = lse2_5(blank2 + buf[CUR][s], mv.x + bs.x, mv.y + bs.y, mv.z + bs.z, mv.w + bs.w) - b0;
+            const float v = lse2_5(stay_cur + buf[CUR][s], mv.x + bs.x, mv.y + bs.y, mv.z + bs.z, mv.w + bs.w) - b0;
+            if constexpr (LB) stay_cur = stay_next;
             buf[CUR ^ 1][s] = v;
             *beta_p = v;
             beta_p -= S;
@@ -199,10 +242,14 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
         // score row t and beta' row t+1 of step t live in slot t % PF of the rings; PF-1 steps are kept in flight
         for (int r = 0; r < PF - 1; ++r) {
             if (r < T) {
-                cp_async_8(&sc_ring[r][s], sc + (size_t)r * S);
+                fetch_row(r);
                 cp_async_4(&beta_ring[r][s], beta + (size_t)(r + 1) * S + s);
             }
             cp_async_commit();
+        }
+        if constexpr (LB) {                                   // row 0, complete and published before step 0
+            cp_async_wait<PF - 2>();
+            __syncthreads();
         }
         double bs_next2 = (T > 1 && s == 0) ? bsum[2] : 0.0;   // thread 0: bsum[t+2], for the normaliser of step t+1
         const double* bsum_p = bsum + 3;
@@ -214,18 +261,29 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
             {
                 const int r = t + PF - 1;
                 if (r < T) {
-                    cp_async_8(&sc_ring[r & (PF - 1)][s], sc + (size_t)r * S);
+                    fetch_row(r);
                     cp_async_4(&beta_ring[r & (PF - 1)][s], beta + (size_t)(r + 1) * S + s);
                 }
                 cp_async_commit();
                 if (s == 0 && t + 3 <= T) bs_n = *bsum_p;
-                cp_async_wait<PF - 1>();
+                // LB: row t+1 as well, published for the next step by the barrier of this one
+                if constexpr (LB) cp_async_wait<PF - 2>();
+                else cp_async_wait<PF - 1>();
             }
             ++bsum_p;
-            const uint2 mraw = sc_ring[t & (PF - 1)][s];
             const float bnext = beta_ring[t & (PF - 1)][s];
-            const float2 m01 = __half22float2(*reinterpret_cast<const __half2*>(&mraw.x));
-            const float2 m23 = __half22float2(*reinterpret_cast<const __half2*>(&mraw.y));
+            float2 m01, m23;
+            float stay2 = blank2;
+            if constexpr (LB) {
+                const __half* e = lb_row(t & (PF - 1));
+                stay2 = __half2float(e[0]) * LOG2E;
+                m01 = make_float2(__half2float(e[1]), __half2float(e[2]));
+                m23 = make_float2(__half2float(e[3]), __half2float(e[4]));
+            } else {
+                const uint2 mraw = sc_ring[t & (PF - 1)][s];
+                m01 = __half22float2(*reinterpret_cast<const __half2*>(&mraw.x));
+                m23 = __half22float2(*reinterpret_cast<const __half2*>(&mraw.y));
+            }
             const float2 a0v0 = av[CUR][0];
             const float kt = kt_sh[CUR];
             float2 p[5];
@@ -233,7 +291,7 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
 #pragma unroll
             for (int j = 0; j < 4; ++j) p[1 + j] = av[CUR][j * Q + pq];
             float x[5];
-            x[0] = p[0].x + blank2;
+            x[0] = p[0].x + stay2;
             x[1] = fmaf(m01.x, LOG2E, p[1].x);
             x[2] = fmaf(m01.y, LOG2E, p[2].x);
             x[3] = fmaf(m23.x, LOG2E, p[3].x);
@@ -345,7 +403,7 @@ crf_decode_kernel(const __half* __restrict__ scores, int T, float blank, float q
 
 inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 
-template <int S>
+template <int S, bool LB = false>
 int launch_decode(const __half* scores, int N, int T, float blank, float qscale, float qbias, void* workspace,
                   uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream) {
     unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
@@ -354,13 +412,13 @@ int launch_decode(const __half* scores, int N, int T, float blank, float qscale,
     double* bsum = reinterpret_cast<double*>(ws + off); off += align256((size_t)N * (T + 1) * sizeof(double));
     float* pm = reinterpret_cast<float*>(ws + off); off += align256((size_t)N * T * 4 * sizeof(float));
     uint8_t* bp = ws + off;
-    size_t dyn = DecodeSmem<S>::bytes(T);
+    size_t dyn = DecodeSmem<S, LB>::bytes(T);
     // B200_DECODE_SMEM_KB pads the request to bound the CTAs per SM (room for a co-resident recurrent CTA)
     if (const char* pad = getenv("B200_DECODE_SMEM_KB")) {
         const size_t want = (size_t)atoi(pad) * 1024;
         if (want > dyn && want <= 200 * 1024) dyn = want;
     }
-    auto kern = crf_decode_kernel<S>;
+    auto kern = crf_decode_kernel<S, LB>;
     B200_REQUIRE(dyn <= 200 * 1024, "crf_decode: chunk of %d frames needs %zu B of shared memory", T, dyn);
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
     kern<<<N, S, dyn, stream>>>(scores, T, blank, qscale, qbias, beta, bsum, bp, pm, moves, seq, qual);
@@ -598,6 +656,19 @@ int launch_crf_decode(const __half* scores, int N, int T, int state_len, float b
         case 5: return launch_decode<1024>(scores, N, T, blank, qscale, qbias, workspace, moves, seq, qual, stream);
         default:
             b200_set_error("crf_decode: state_len %d is not supported (3, 4, 5)", state_len);
+            return -2;
+    }
+}
+
+int launch_crf_decode_lb(const __half* scores, int N, int T, int state_len, float qscale, float qbias, void* workspace,
+                         uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream) {
+    if (N == 0 || T == 0) return 0;
+    switch (state_len) {
+        case 3: return launch_decode<64, true>(scores, N, T, 0.f, qscale, qbias, workspace, moves, seq, qual, stream);
+        case 4: return launch_decode<256, true>(scores, N, T, 0.f, qscale, qbias, workspace, moves, seq, qual, stream);
+        case 5: return launch_decode<1024, true>(scores, N, T, 0.f, qscale, qbias, workspace, moves, seq, qual, stream);
+        default:
+            b200_set_error("crf_decode_lb: state_len %d is not supported (3, 4, 5)", state_len);
             return -2;
     }
 }

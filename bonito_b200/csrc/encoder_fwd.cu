@@ -7,7 +7,7 @@
 
 int launch_conv_stem(const __half* x, int N, int L, int C1, int K1, const __half* w1, const __half* b1, int act1,
                      int C2, int K2, const __half* w2, const __half* b2, int act2, __half* out, int Lp, int padl,
-                     cudaStream_t stream);
+                     float lo1, float hi1, float lo2, float hi2, cudaStream_t stream);
 int launch_lstm_rec_tile(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
                          int reverse, cudaStream_t stream);
 int lstm_rec_tile_chunks(int hidden);
@@ -21,6 +21,9 @@ int launch_lstm_crf_fwd(const b200_lstm_crf_plan* p, const __half* x, __half* sc
     B200_REQUIRE(p->n_lstm >= 1 && p->n_lstm <= B200_MAX_LSTM_LAYERS, "lstm_crf_fwd: %d LSTM layers are not supported", p->n_lstm);
     const int N = p->n, L = p->l, T = p->t, Tp = p->tp, Lp = Tp * p->s3, CW = 4 * H / CS;
     B200_REQUIRE(N > 0 && L > 0 && T > 0 && Tp >= T, "lstm_crf_fwd: bad geometry n=%d l=%d t=%d tp=%d", N, L, T, Tp);
+    // the plan carries no bounds for the convolutions: clamped activations go through the layer-by-layer entry points
+    B200_REQUIRE(p->act1 != B200_ACT_SWISH_CLAMP && p->act2 != B200_ACT_SWISH_CLAMP && p->act3 != B200_ACT_SWISH_CLAMP,
+                 "lstm_crf_fwd: B200_ACT_SWISH_CLAMP needs bounds the plan does not carry");
     const int nt = (N + TB - 1) / TB;
     __half* stem = (__half*)p->stem;
     __half* cur = (__half*)p->ya;
@@ -28,7 +31,8 @@ int launch_lstm_crf_fwd(const b200_lstm_crf_plan* p, const __half* x, __half* sc
     __half* gx = (__half*)p->gx;
 
     int rc = launch_conv_stem(x, N, L, p->c1, p->k1, (const __half*)p->w1, (const __half*)p->b1, p->act1, p->c2, p->k2,
-                              (const __half*)p->w2, (const __half*)p->b2, p->act2, stem, Lp, p->pad3, stream);
+                              (const __half*)p->w2, (const __half*)p->b2, p->act2, stem, Lp, p->pad3, 0.f, 0.f, 0.f, 0.f,
+                              stream);
     if (rc) return rc;
     GemmEpilogue ep;
     // strided convolution: rows r = n*Tp + t are windows of k3*c2 elements, s3*c2 apart -> ya[tile n/TB][t][n%TB]

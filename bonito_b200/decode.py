@@ -20,20 +20,22 @@ import os
 import numpy as np
 import torch
 
-from bonito_b200.engine import CrfDecoder
+from bonito_b200.engine import CrfDecoder, score_layout
 
 _decoder = CrfDecoder()
 
 
 def beam_search(scores, beam_width=32, beam_cut=100.0, scale=1.0, offset=0.0, blank_score=2.0, decoder=None):
     """
-    scores: CUDA fp16 [N, T, 4**(k+1)] contiguous (no blank column).
+    scores: CUDA fp16 contiguous, either [N, T, 4**(k+1)] (fixed blank: no blank column, [state][m0..m3], the stay score is
+    `blank_score`) or [N, T, 5 * 4**k] (learned blank scores: the CTC_CRF layout [state][stay, m0..m3]; `blank_score` is
+    ignored).  The width picks the layout and k.  The beam search (`decoder="beam"`) needs a fixed blank score.
     Returns (sequence, qstring, moves): three CPU uint8 tensors [N, T]; sequence / qstring carry an
     ASCII character on frames that emit a base and 0 elsewhere.  `scale` / `offset` are the qscore
     scale and bias (q = -10 log10(max(1-p, 1e-4)) * scale + offset).
     """
     n, t, c = scores.shape
-    state_len = int(round(np.log(c) / np.log(4))) - 1
+    state_len, _ = score_layout(c)
     decoder = decoder or os.environ.get("B200_DECODER", "exact")
     if decoder not in ("exact", "beam"):
         raise ValueError(f"unknown decoder {decoder!r} (exact, beam)")

@@ -6,14 +6,18 @@ Plan builder + executor for the LSTM-CRF encoder (the `bonito.crf` fast / hac / 
 configs describe (`bonito/models/configs/dna_r10.4.1@v4.3.toml`,
 `bonito/crf/model.py:150-162`):
 
-    Convolution(1->C1,k5) , Convolution(C1->C2,k5) , Convolution(C2->H,kW,stride s)
-    Permute([2,0,1]) , LSTM x L (alternating reverse) , LinearCRFEncoder [, Clamp]
+    Convolution(1->C1,k5) [, Clamp] , Convolution(C1->C2,k5) [, Clamp] , Convolution(C2->H,kW,stride s) [, Clamp]
+    Permute([2,0,1]) , LSTM x L (alternating reverse) [, Linear(H->B)] , LinearCRFEncoder [, Clamp]
 
 (LinearCRFEncoder: a plain linear head followed by a Clamp layer, as in the v4+ configs, or the old-style head with
-activation = "tanh" and / or a scale and no Clamp; fixed blank_score) and packs the weights into the operand layouts of
-the sm_90a kernels (include/bonito_b200.h).  This is the native swap-in the reference performs in `Model.use_koi`
+activation = "tanh" and / or a scale and no Clamp) and packs the weights into the operand layouts of the sm_90a kernels
+(include/bonito_b200.h).  This is the native swap-in the reference performs in `Model.use_koi`
 (`bonito/crf/model.py:240-246`, koi.lstm.update_graph); like koi it returns scores as `[N, T, C]` fp16 without the blank
-column.  Anything else raises `UnsupportedModel`.
+column when the head has a fixed blank_score.  A head without one (dna_r9.4.1@v3) learns its blank scores: the scores
+are then `[N, T, 5 * 4^k]` in the CTC_CRF order [state][stay, m0..m3] (b200_crf_decode_lb).  A Clamp behind a (swish)
+convolution (dna_r10.4.1@v4.0) is fused into its epilogue (B200_ACT_SWISH_CLAMP), the Linear in front of the head is one
+more GEMM; these layers and learned blank scores run on the wide path (H = 768, 1024) only.  Anything else raises
+`UnsupportedModel`.
 
 Width 384 (hac), the headline path (`forward_tiles`): activations tile-major `[tile][T][64][H]`, gate pre-activations
 `[tile][T][8][64][192]`; per layer ONE input GEMM over all tiles and ONE launch of the recurrent kernel (one 8-CTA
@@ -28,7 +32,7 @@ pipelined on per-tile streams; `B200_LSTM_TILE=0` sends width 384 down this path
 Widths 768 and 1024 (`forward_wide`: dna_r9.4.1@v3.1, dna_r10.4.1@v4.3): W_hh does not fit the shared memory of one cluster,
 so the recurrence runs on the grid-wide kernel (lstm_rec_wide.cu: H / 8 co-resident CTAs, one cooperative launch per layer);
 activations `[T][N][H]`, gate pre-activations `[T][H/8][N][32]`, layer by layer on the current stream, one buffer set (no
-slots), no int8 input projection.
+slots), no int8 input projection; the output of the Linear in front of the head, if any, is `[T][N][B]`.
 """
 
 import torch
@@ -61,6 +65,52 @@ def _folded_conv(layer):
             raise UnsupportedModel(f"norm {layer.norm!r} has no native kernel")
         conv = torch.nn.utils.fusion.fuse_conv_bn_eval(conv.eval(), layer.norm.bn.eval())
     return conv.weight.detach(), None if conv.bias is None else conv.bias.detach()
+
+
+def _conv_act(conv, clamp):
+    """(activation code, lo, hi) of a Convolution and the Clamp layer behind it (None: no Clamp)."""
+    act = _act_code(conv.activation)
+    if clamp is None:
+        return act, 0.0, 0.0
+    if act != native.ACT_SWISH:
+        raise UnsupportedModel(f"a Clamp after a convolution is supported behind a swish activation; got {conv.activation!r}")
+    return native.ACT_SWISH_CLAMP, float(clamp.min), float(clamp.max)
+
+
+def _parse_stack(layers):
+    """
+    Split an encoder into (convs, clamps behind them, lstms, bottleneck Linear or None, LinearCRFEncoder, head clamps) if it is
+        [Convolution, Clamp?] x 3, Permute([2, 0, 1]), LSTM x L (L >= 1), Linear?, LinearCRFEncoder, Clamp?
+    and raise UnsupportedModel otherwise.
+    """
+    names = [type(m).__name__ for m in layers]
+    err = UnsupportedModel("native LSTM-CRF path needs [Convolution, Clamp?] x 3, Permute([2, 0, 1]), LSTM x L, Linear?, "
+                           f"LinearCRFEncoder, Clamp?; got {names}")
+    i = 0
+
+    def take(cls):
+        nonlocal i
+        if i < len(layers) and isinstance(layers[i], cls):
+            i += 1
+            return layers[i - 1]
+        return None
+
+    convs, conv_clamps = [], []
+    for _ in range(3):
+        convs.append(take(bnn.Convolution))
+        conv_clamps.append(take(bnn.Clamp))
+    permute = take(bnn.Permute)
+    if None in convs or permute is None or list(permute.dims) != [2, 0, 1]:
+        raise err
+    lstms = []
+    while (m := take(bnn.LSTM)) is not None:
+        lstms.append(m)
+    bottleneck = take(bnn.Linear)
+    crf = take(bnn.LinearCRFEncoder)
+    head_clamp = take(bnn.Clamp)
+    if not lstms or crf is None or i != len(layers):
+        raise err
+    return convs, conv_clamps, lstms, bottleneck, crf, [] if head_clamp is None else [head_clamp]
 
 
 def _dev16(t, device):
@@ -110,16 +160,7 @@ class LstmCrfPlan:
     """Packed weights + cached buffers for one LSTM-CRF encoder on one device."""
 
     def __init__(self, encoder, device, quantize=False):
-        layers = list(encoder.children())
-        convs = [m for m in layers if isinstance(m, bnn.Convolution)]
-        lstms = [m for m in layers if isinstance(m, bnn.LSTM)]
-        crfs = [m for m in layers if isinstance(m, bnn.LinearCRFEncoder)]
-        clamps = [m for m in layers if isinstance(m, bnn.Clamp)]
-        others = [m for m in layers if not isinstance(
-            m, (bnn.Convolution, bnn.LSTM, bnn.LinearCRFEncoder, bnn.Clamp, bnn.Permute))]
-        if len(convs) != 3 or not lstms or len(crfs) != 1 or others or len(clamps) > 1:
-            raise UnsupportedModel("native LSTM-CRF path needs 3 convolutions, >=1 LSTM, one LinearCRFEncoder "
-                                   f"and at most one Clamp; got {[type(m).__name__ for m in layers]}")
+        convs, conv_clamps, lstms, bottleneck, crf, clamps = _parse_stack(list(encoder.children()))
         self.device = torch.device(device)
 
         # --- conv stem (conv1 + conv2) -------------------------------------------------------
@@ -130,17 +171,21 @@ class LstmCrfPlan:
                 raise UnsupportedModel("conv stem layers must be stride 1 with 'same' padding")
         if c1.conv.in_channels != 1:
             raise UnsupportedModel("the encoder must take a single input feature")
+        (self.act1, lo1, hi1), (self.act2, lo2, hi2), (self.act3, self.lo3, self.hi3) = (
+            _conv_act(c, clamp) for c, clamp in zip(convs, conv_clamps))
+        # bounds of the stem activations (B200_ACT_SWISH_CLAMP), None: no clamp in the stem
+        self.stem_bounds = (lo1, hi1, lo2, hi2) if any(conv_clamps[:2]) else None
         w1, b1 = _folded_conv(c1)
         w2, b2 = _folded_conv(c2)
-        self.w1, self.b1, self.act1 = _dev16(w1, device), _dev16(b1, device), _act_code(c1.activation)
-        self.w2, self.b2, self.act2 = _dev16(w2, device), _dev16(b2, device), _act_code(c2.activation)
+        self.w1, self.b1 = _dev16(w1, device), _dev16(b1, device)
+        self.w2, self.b2 = _dev16(w2, device), _dev16(b2, device)
 
         # --- strided conv as GEMM: weight [H][C2][K3] -> [H][K3*C2], k = tap*C2 + cin -------
         w3, b3 = _folded_conv(c3)
         self.hidden, self.c2, self.k3 = w3.shape
         self.s3, self.pad3 = c3.conv.stride[0], c3.conv.padding[0]
         self.w3 = _dev16(w3.permute(0, 2, 1).reshape(self.hidden, -1), device)
-        self.b3, self.act3 = _dev16(b3, device), _act_code(c3.activation)
+        self.b3 = _dev16(b3, device)
         if (self.k3 * self.c2) % 8 or (self.s3 * self.c2) % 8:
             raise UnsupportedModel("strided conv window/stride must be multiples of 8 elements")
 
@@ -188,20 +233,39 @@ class LstmCrfPlan:
         if self.quantize and not (self.tile and H % 16 == 0):
             raise UnsupportedModel("the int8 input projection (--quantize) needs the tile-layout LSTM path (hidden size 384)")
 
+        # --- bottleneck Linear(H -> B) in front of the head (dna_r10.4.1@v4.0) ----------------------
+        self.wb = self.bb = None
+        self.head_in = H                                    # input width of the CRF head GEMM
+        if bottleneck is not None:
+            lin = bottleneck.linear
+            if lin.in_features != H or lin.out_features % 8:
+                raise UnsupportedModel(f"the Linear in front of the CRF head must map the LSTM width {H} to a multiple of 8 "
+                                       f"features; got {lin.in_features} -> {lin.out_features}")
+            self.wb = _dev16(lin.weight.detach(), device)
+            self.bb = _dev16(None if lin.bias is None else lin.bias.detach(), device)
+            self.head_in = lin.out_features
+
         # --- linear CRF head (+ clamp) ---------------------------------------------------------
-        crf = crfs[0]
         if crf.permute is not None:
             raise UnsupportedModel("native LinearCRFEncoder supports permute=None")
         crf_act = _act_code(crf.activation)
         if crf_act not in (native.ACT_NONE, native.ACT_TANH) or ((crf_act != native.ACT_NONE or crf.scale is not None) and clamps):
             raise UnsupportedModel("native LinearCRFEncoder supports tanh and / or a scale (old-style configs), or a Clamp layer "
                                    "behind a plain linear head (v4+ configs)")
-        if crf.blank_score is None:
-            raise UnsupportedModel("native decode needs a fixed blank_score")
-        self.n_base, self.state_len, self.blank_score = crf.n_base, crf.state_len, float(crf.blank_score)
+        self.n_base, self.state_len = crf.n_base, crf.state_len
+        # blank_score None: learned blank scores, the head emits [state][stay, m0..m3] (5 * 4^k columns, b200_crf_decode_lb)
+        self.blank_score = None if crf.blank_score is None else float(crf.blank_score)
         self.wl = _dev16(crf.linear.weight.detach(), device)
         self.bl = _dev16(None if crf.linear.bias is None else crf.linear.bias.detach(), device)
         self.n_scores = self.wl.shape[0]
+        if self.wl.shape[1] != self.head_in:
+            raise UnsupportedModel(f"the CRF head takes {self.wl.shape[1]} features; the layer before it gives {self.head_in}")
+        new_layers = [name for name, used in (("a Clamp after a convolution", any(conv_clamps)),
+                                              ("a Linear in front of the CRF head", bottleneck is not None),
+                                              ("learned blank scores", self.blank_score is None)) if used]
+        if new_layers and not self.wide:
+            raise UnsupportedModel(f"{' and '.join(new_layers)} run on the wide LSTM path only (hidden size 768 or 1024); "
+                                   f"this model has hidden size {H}")
         if clamps:
             self.act_l, self.lo, self.hi = native.ACT_CLAMP, float(clamps[0].min), float(clamps[0].max)
         elif crf_act == native.ACT_TANH and crf.scale is not None:     # e.g. the dna_r9.4.1 configs: tanh, scale 5.0
@@ -585,6 +649,7 @@ class LstmCrfPlan:
                 ya=torch.empty(T, N, H, dtype=f16, device=dev),
                 yb=torch.empty(T, N, H, dtype=f16, device=dev),
                 gx=torch.empty(T, self.wide, N, 4 * H // self.wide, dtype=f16, device=dev),
+                yl=None if self.wb is None else torch.empty(T, N, self.head_in, dtype=f16, device=dev),
                 ws=ws, ws_status=ws[off:off + 4].view(torch.int32),
                 status=torch.zeros(len(self.lstm), dtype=torch.int32, device=dev),
             )
@@ -633,13 +698,15 @@ class LstmCrfPlan:
             return _Stage(name, events)
 
         with stage("conv_stem"):
-            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3)
+            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3,
+                             bounds=self.stem_bounds)
         if return_features:
             feats["stem"] = b["stem"][:N * Lp * self.c2].view(N, Lp, self.c2)[:, self.pad3:self.pad3 + L].clone()
         cur, nxt = b["ya"], b["yb"]
         with stage("conv_gemm"):
             native.gemm(b["stem"], self.s3 * self.c2, self.w3, self.b3, cur, H, N * Tp, H, self.k3 * self.c2,
-                        act=self.act3, rows_inner=Tp, valid_inner=T, stride_inner=N, stride_outer=1, impl=gemm_impl)
+                        act=self.act3, lo=self.lo3, hi=self.hi3, rows_inner=Tp, valid_inner=T, stride_inner=N, stride_outer=1,
+                        impl=gemm_impl)
         if return_features:
             feats["conv"] = cur.clone()
         for i, layer in enumerate(self.lstm):
@@ -652,11 +719,17 @@ class LstmCrfPlan:
             cur, nxt = nxt, cur
             if return_features:
                 feats[f"lstm{i}"] = cur.clone()
+        if self.wb is not None:
+            with stage("bottleneck_gemm"):  # rows r = t*N + n -> yl[t][n][:]
+                native.gemm(cur, H, self.wb, self.bb, b["yl"], self.head_in, T * N, self.head_in, H, impl=gemm_impl)
+            cur = b["yl"]
+            if return_features:
+                feats["linear"] = cur.clone()
 
         if out is None:
             out = torch.empty(N, T, self.n_scores, dtype=torch.float16, device=self.device)
         with stage("crf_gemm"):             # rows r = t*N + n -> out[n][t][:]
-            native.gemm(cur, H, self.wl, self.bl, out, self.n_scores, T * N, self.n_scores, H,
+            native.gemm(cur, self.head_in, self.wl, self.bl, out, self.n_scores, T * N, self.n_scores, self.head_in,
                         act=self.act_l, lo=self.lo, hi=self.hi,
                         rows_inner=N, valid_inner=N, stride_inner=T, stride_outer=1, impl=gemm_impl)
         status = torch.empty(len(self.lstm), dtype=torch.int32, pin_memory=True)
@@ -792,24 +865,40 @@ def compile_lstm_crf(encoder, device, quantize=False):
     return LstmCrfPlan(encoder, device, quantize=quantize)
 
 
+def score_layout(width, state_len=None):
+    """(state_len, learned_blank) of CRF scores `width` columns wide: 4**(k+1) = moves only, the fixed-blank layout
+    [state][m0..m3]; 5 * 4**k = learned blanks, the CTC_CRF layout [state][stay, m0..m3].  The two never coincide.
+    `state_len`: the model's, checked against the width; None: inferred from it."""
+    for k in ((state_len,) if state_len is not None else range(1, 9)):
+        if width == 4 ** (k + 1):
+            return k, False
+        if width == 5 * 4 ** k:
+            return k, True
+    raise ValueError(f"scores width {width} is neither 4**(k+1) (fixed blank) nor 5 * 4**k (learned blank)"
+                     + ("" if state_len is None else f" for state_len {state_len}"))
+
+
 class CrfDecoder:
-    """Workspace-caching wrapper around b200_crf_decode."""
+    """Workspace-caching wrapper around b200_crf_decode (fixed blank: scores [N, T, 4**(k+1)], [state][m0..m3]) and
+    b200_crf_decode_lb (learned blank: scores [N, T, 5 * 4**k], [state][stay, m0..m3]); the score width picks the kernel."""
 
     def __init__(self):
         self._ws_by_device = {}     # one workspace per (device, host thread): basecall() decodes on background threads
 
     def __call__(self, scores, state_len, blank_score=2.0, qscale=1.0, qbias=0.0, events=None, out=None, slot=0, beam=None):
         """`beam=(beam_width, beam_cut)`: run the beam search (after the forward-backward pass) instead of the exact
-        posterior-Viterbi trace-back."""
+        posterior-Viterbi trace-back (fixed blank only).  `blank_score` is ignored for learned-blank scores."""
         with torch.cuda.device(scores.device):
             return self._call(scores, state_len, blank_score, qscale, qbias, events, out, slot, beam)
 
     def _call(self, scores, state_len, blank_score, qscale, qbias, events, out, slot=0, beam=None):
         """-> (moves, sequence, qstring) uint8 [N, T] on the device; `out`: optional uint8 [3, N, T] to write them into."""
         n, t, c = scores.shape
-        if c != 4 ** (state_len + 1):
-            raise ValueError(f"scores width {c} does not match state_len {state_len}")
-        cached = DECODE_CACHE.take(scores, (state_len, float(blank_score), float(qscale), float(qbias)))
+        _, learned = score_layout(c, state_len)
+        if learned and beam is not None:
+            raise ValueError("the beam search kernel needs a fixed blank score; scores with learned blank scores "
+                             "(5 * 4**state_len columns) decode with the exact decoder only")
+        cached = None if learned else DECODE_CACHE.take(scores, (state_len, float(blank_score), float(qscale), float(qbias)))
         if cached is not None:
             if out is not None:
                 for dst, src in zip(out, cached):
@@ -825,7 +914,9 @@ class CrfDecoder:
             ws = self._ws_by_device[key] = torch.empty(need, dtype=torch.uint8, device=scores.device)
         outs = list(out) if out is not None else [torch.empty(n, t, dtype=torch.uint8, device=scores.device) for _ in range(3)]
         with _Stage("crf_decode", events):
-            if beam is None:
+            if learned:
+                native.crf_decode_lb(scores, state_len, qscale, qbias, ws, *outs)
+            elif beam is None:
                 native.crf_decode(scores, state_len, blank_score, qscale, qbias, ws, *outs)
             else:
                 native.crf_beam_search(scores, state_len, blank_score, beam[0], beam[1], qscale, qbias, ws, *outs)

@@ -15,7 +15,7 @@ import torch
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libbonito_b200.so")
 _lib = None
 
-ACT_NONE, ACT_SWISH, ACT_TANH, ACT_CLAMP, ACT_SCALE, ACT_SWIGLU, ACT_TANH_SCALE = 0, 1, 2, 3, 4, 5, 6
+ACT_NONE, ACT_SWISH, ACT_TANH, ACT_CLAMP, ACT_SCALE, ACT_SWIGLU, ACT_TANH_SCALE, ACT_SWISH_CLAMP = 0, 1, 2, 3, 4, 5, 6, 7
 GEMM_AUTO, GEMM_TCGEN05, GEMM_MMA_SYNC = 0, 1, 2
 
 MAX_LSTM_LAYERS = 8
@@ -41,6 +41,9 @@ SIGNATURES = {
     "b200_last_error": (c_char_p, []),
     "b200_conv_stem_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                    c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "b200_conv_stem_fwd_ex": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_float,
+                                      c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_float, c_void_p, c_int, c_int,
+                                      c_void_p]),
     "b200_gemm_fwd": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int,
                               c_int, c_float, c_float, c_int, c_int, c_longlong, c_longlong, c_int, c_void_p]),
     "b200_gemm_fwd_ex": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int,
@@ -77,6 +80,8 @@ SIGNATURES = {
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_crf_decode": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_float,
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_crf_decode_lb": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float,
+                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 
@@ -137,15 +142,22 @@ def version():
     return load().b200_version()
 
 
-def conv_stem(x, w1, b1, act1, w2, b2, act2, out, lp, padl):
-    """x [N,L] -> out [N,lp,C2] channels-last, zero padded (see b200_conv_stem_fwd)."""
+def conv_stem(x, w1, b1, act1, w2, b2, act2, out, lp, padl, bounds=None):
+    """x [N,L] -> out [N,lp,C2] channels-last, zero padded (see b200_conv_stem_fwd).  `bounds=(lo1, hi1, lo2, hi2)`: the
+    bounds of act1 / act2 (B200_ACT_SWISH_CLAMP), through b200_conv_stem_fwd_ex."""
     lib = require()
     n, l = x.shape
     c1, _, k1 = w1.shape
     c2, _, k2 = w2.shape
     with torch.cuda.device(x.device):
-        rc = lib.b200_conv_stem_fwd(_ptr(_f16(x, "x")), n, l, c1, k1, _ptr(_f16(w1, "w1")), _ptr(b1), act1,
-                                    c2, k2, _ptr(_f16(w2, "w2")), _ptr(b2), act2, _ptr(out), lp, padl, _stream())
+        if bounds is None:
+            rc = lib.b200_conv_stem_fwd(_ptr(_f16(x, "x")), n, l, c1, k1, _ptr(_f16(w1, "w1")), _ptr(b1), act1,
+                                        c2, k2, _ptr(_f16(w2, "w2")), _ptr(b2), act2, _ptr(out), lp, padl, _stream())
+        else:
+            lo1, hi1, lo2, hi2 = (float(v) for v in bounds)
+            rc = lib.b200_conv_stem_fwd_ex(_ptr(_f16(x, "x")), n, l, c1, k1, _ptr(_f16(w1, "w1")), _ptr(b1), act1, lo1, hi1,
+                                           c2, k2, _ptr(_f16(w2, "w2")), _ptr(b2), act2, lo2, hi2, _ptr(out), lp, padl,
+                                           _stream())
     _check(rc, "b200_conv_stem_fwd")
     return out
 
@@ -296,6 +308,18 @@ def crf_decode(scores, state_len, blank_score, qscale, qbias, workspace, moves, 
                                  float(qbias), _ptr(workspace), _ptr(moves), _ptr(sequence), _ptr(qstring),
                                  _stream(stream))
     _check(rc, "b200_crf_decode")
+    return moves, sequence, qstring
+
+
+def crf_decode_lb(scores, state_len, qscale, qbias, workspace, moves, sequence, qstring, stream=None):
+    """Learned-blank decode (see b200_crf_decode_lb): scores [N, T, 5 * 4**state_len] in the [state][stay, m0..m3] layout;
+    workspace of crf_decode_workspace_bytes(N, T, state_len) bytes."""
+    lib = require()
+    n, t, _ = scores.shape
+    with torch.cuda.device(scores.device):
+        rc = lib.b200_crf_decode_lb(_ptr(scores), n, t, state_len, float(qscale), float(qbias), _ptr(workspace), _ptr(moves),
+                                    _ptr(sequence), _ptr(qstring), _stream(stream))
+    _check(rc, "b200_crf_decode_lb")
     return moves, sequence, qstring
 
 

@@ -32,21 +32,33 @@ def model_spec(name="hac", n_lstm=5, stride=6, winlen=19):
     )
 
 
-def old_style_spec(n_lstm=5):
+def v40_spec(n_lstm=5):
+    """dna_r10.4.1@v4.0, the R10.4.1 LSTM sup model before v4.3: the v4.3 stack at width 1024 with Clamp(-0.5, 3.5) behind
+    each of the three convolutions, conv3 stride 5 with swish, and a Linear 1024 -> 256 (with bias) in front of the head."""
+    spec = model_spec("sup_lstm", n_lstm=n_lstm, stride=5)
+    spec["convs"][2] = (16, 1024, 19, 5, 9, "swish")
+    spec.update(name="sup_lstm_v40", conv_clamp=(-0.5, 3.5), bottleneck=256)
+    return spec
+
+
+def old_style_spec(n_lstm=5, blank_score=2.0):
     """dna_r9.4.1@v3.1: the old-style `[encoder]` (built by rnn_encoder, bonito/crf/model.py:150-162): 1 -> 4 -> 16 stem,
-    conv3 k19 stride 5 swish into width 768, LSTMs reversed (n_lstm - i) % 2, LinearCRFEncoder with bias, tanh, scale 5."""
+    conv3 k19 stride 5 swish into width 768, LSTMs reversed (n_lstm - i) % 2, LinearCRFEncoder with bias, tanh, scale 5.
+    `blank_score=None`: dna_r9.4.1@v3, whose head learns its blank scores ((n_base + 1) * 4^state_len outputs)."""
     return dict(
-        name="r9_v3.1", hidden=768, state_len=5, n_lstm=n_lstm,
+        name="r9_v3.1" if blank_score is not None else "r9_v3", hidden=768, state_len=5, n_lstm=n_lstm,
         convs=[(1, 4, 5, 1, 2, "swish"), (4, 16, 5, 1, 2, "swish"), (16, 768, 19, 5, 9, "swish")],
         reverse=[bool((n_lstm - i) % 2) for i in range(n_lstm)],
-        blank_score=2.0, clamp=None, stride=5, crf_activation="tanh", crf_scale=5.0, crf_bias=True, old_style=True,
+        blank_score=blank_score, clamp=None, stride=5, crf_activation="tanh", crf_scale=5.0, crf_bias=True, old_style=True,
     )
 
 
 def old_style_config(spec, batchsize=32, chunksize=4000, overlap=500):
     """TOML-equivalent dict of an old-style config (the keys of dna_r9.4.1@v3.1.toml)."""
     enc = dict(stride=spec["convs"][2][3], winlen=spec["convs"][2][2], scale=spec["crf_scale"], features=spec["hidden"],
-               rnn_type="lstm", activation=spec["convs"][2][5], blank_score=spec["blank_score"])
+               rnn_type="lstm", activation=spec["convs"][2][5])
+    if spec["blank_score"] is not None:                 # dna_r9.4.1@v3 has no blank_score key: learned blank scores
+        enc["blank_score"] = spec["blank_score"]
     if spec["n_lstm"] != 5:
         enc["num_layers"] = spec["n_lstm"]
     return {
@@ -61,7 +73,8 @@ def old_style_config(spec, batchsize=32, chunksize=4000, overlap=500):
 
 
 def model_config(spec, batchnorm=False, batchsize=32, chunksize=3996, overlap=492):
-    """TOML-equivalent dict for `Model(config)` (layout of dna_r10.4.1@v4.3.toml; `old_style_config` for old_style specs)."""
+    """TOML-equivalent dict for `Model(config)` (layout of dna_r10.4.1@v4.3.toml, and of @v4.0.toml for specs with
+    `conv_clamp` / `bottleneck`; `old_style_config` for old_style specs)."""
     if spec.get("old_style"):
         return old_style_config(spec, batchsize=batchsize, chunksize=chunksize, overlap=overlap)
     sub = []
@@ -70,11 +83,17 @@ def model_config(spec, batchnorm=False, batchsize=32, chunksize=3996, overlap=49
         if batchnorm:
             layer["norm"] = "batchnorm"
         sub.append(layer)
+        if spec.get("conv_clamp") is not None:
+            sub.append(dict(type="clamp", min=spec["conv_clamp"][0], max=spec["conv_clamp"][1]))
     sub.append(dict(type="permute", dims=[2, 0, 1]))
     for i in range(spec["n_lstm"]):
         sub.append(dict(type="lstm", size=spec["hidden"], insize=spec["hidden"], bias=True, reverse=int(spec["reverse"][i])))
-    crf = dict(type="linearcrfencoder", insize=spec["hidden"], n_base=4, state_len=spec["state_len"], bias=False,
-               blank_score=spec["blank_score"])
+    if spec.get("bottleneck") is not None:
+        sub.append(dict(type="linear", in_features=spec["hidden"], out_features=spec["bottleneck"]))
+    crf = dict(type="linearcrfencoder", insize=spec.get("bottleneck") or spec["hidden"], n_base=4,
+               state_len=spec["state_len"], bias=False)
+    if spec["blank_score"] is not None:
+        crf["blank_score"] = spec["blank_score"]
     if spec.get("crf_activation") is not None:          # old-style head: tanh + scale instead of a Clamp layer
         crf["activation"] = spec["crf_activation"]
     if spec.get("crf_scale") is not None:
@@ -105,7 +124,8 @@ def _orthogonal_blocks(rows, cols, block, gen, gain, f64=False):
     return w * gain
 
 
-def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp16_values=True, qr_f64=False):
+def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp16_values=True, qr_f64=False,
+                 bottleneck_gain=1.0, blank_gain=0.3, blank_bias=0.4):
     """
     Seeded, non-degenerate weights (oracle naming).  The reference's own init (orthogonal LSTM blocks,
     0.5*truncated-normal input bias, zero state bias: bonito/nn.py:362-390) with gains chosen so that
@@ -115,6 +135,10 @@ def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp1
     With `fp16_values` every tensor is rounded to fp16 (what `model.half()` feeds every implementation).
     `qr_f64=True` factorises the same Gaussian draws in float64: the fp16-rounded weights are then the same on every
     CPU (the float32 QR may round differently elsewhere), for fixtures that store a digest instead of the weights.
+    Specs with a `bottleneck` get `linear.weight` / `linear.bias` (drawn after the LSTMs); with `blank_score=None` the head
+    has 5 * 4^state_len outputs (learned blank scores) and its blank rows are scaled by `blank_gain` and shifted by
+    `blank_bias` (bias, if any): the seeded stacks vary little from frame to frame, and blank rows drawn like the move rows
+    give a few states stay scores near the tanh ceiling that the best path never leaves (one or two bases per chunk).
     """
     gen = torch.Generator().manual_seed(seed)
     H = spec["hidden"]
@@ -128,10 +152,19 @@ def make_weights(spec, seed=25, conv_gain=2.5, lstm_gain=1.5, head_gain=6.0, fp1
         w[f"lstm{i}.w_hh"] = _orthogonal_blocks(4 * H, H, H, gen, lstm_gain, qr_f64)
         w[f"lstm{i}.b_ih"] = 0.5 * torch.randn(4 * H, generator=gen).clamp(-2, 2)
         w[f"lstm{i}.b_hh"] = torch.zeros(4 * H)
-    C = 4 ** (spec["state_len"] + 1)
-    w["crf.weight"] = torch.randn(C, H, generator=gen) * (head_gain / H ** 0.5)
+    head_in = H
+    if spec.get("bottleneck") is not None:
+        head_in = spec["bottleneck"]
+        w["linear.weight"] = torch.randn(head_in, H, generator=gen) * (bottleneck_gain / H ** 0.5)
+        w["linear.bias"] = torch.randn(head_in, generator=gen) * 0.1
+    C = 4 ** (spec["state_len"] + 1) if spec["blank_score"] is not None else 5 * 4 ** spec["state_len"]
+    w["crf.weight"] = torch.randn(C, head_in, generator=gen) * (head_gain / head_in ** 0.5)
     if spec.get("crf_bias"):                 # old-style heads (LinearCRFEncoder default bias=True)
         w["crf.bias"] = torch.randn(C, generator=gen) * 0.1
+    if spec["blank_score"] is None:          # rows [state][stay, m0..m3]
+        w["crf.weight"].view(-1, 5, head_in)[:, 0] *= blank_gain
+        if "crf.bias" in w:
+            w["crf.bias"].view(-1, 5)[:, 0] += blank_bias
     if fp16_values:
         w = {k: v.half().float() for k, v in w.items()}
     return w
@@ -141,18 +174,24 @@ def state_dict_from_weights(spec, weights, prefix="encoder."):
     """Oracle naming -> the module tree's state_dict keys (SURVEY.md Appendix A 'State-dict names')."""
     sd = {}
     n_conv = len(spec["convs"])
+    per_conv = 2 if spec.get("conv_clamp") is not None else 1     # Convolution [, Clamp]
     for i in range(n_conv):
-        sd[f"{prefix}{i}.conv.weight"] = weights[f"conv{i}.weight"]
-        sd[f"{prefix}{i}.conv.bias"] = weights[f"conv{i}.bias"]
-    base = n_conv + 1  # + Permute
+        sd[f"{prefix}{i * per_conv}.conv.weight"] = weights[f"conv{i}.weight"]
+        sd[f"{prefix}{i * per_conv}.conv.bias"] = weights[f"conv{i}.bias"]
+    base = n_conv * per_conv + 1  # + Permute
     for i in range(spec["n_lstm"]):
         sd[f"{prefix}{base + i}.rnn.weight_ih_l0"] = weights[f"lstm{i}.w_ih"]
         sd[f"{prefix}{base + i}.rnn.weight_hh_l0"] = weights[f"lstm{i}.w_hh"]
         sd[f"{prefix}{base + i}.rnn.bias_ih_l0"] = weights[f"lstm{i}.b_ih"]
         sd[f"{prefix}{base + i}.rnn.bias_hh_l0"] = weights[f"lstm{i}.b_hh"]
-    sd[f"{prefix}{base + spec['n_lstm']}.linear.weight"] = weights["crf.weight"]
+    head = base + spec["n_lstm"]
+    if "linear.weight" in weights:
+        sd[f"{prefix}{head}.linear.weight"] = weights["linear.weight"]
+        sd[f"{prefix}{head}.linear.bias"] = weights["linear.bias"]
+        head += 1
+    sd[f"{prefix}{head}.linear.weight"] = weights["crf.weight"]
     if "crf.bias" in weights:
-        sd[f"{prefix}{base + spec['n_lstm']}.linear.bias"] = weights["crf.bias"]
+        sd[f"{prefix}{head}.linear.bias"] = weights["crf.bias"]
     return sd
 
 

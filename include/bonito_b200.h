@@ -5,11 +5,13 @@
  * third-party binaries reached from these call sites, which are what each entry point replaces:
  *
  *   b200_conv_stem_fwd        torch.nn.Conv1d x2 + activations        bonito/nn.py:221-241
+ *                             (_ex: + Clamp behind each, dna_r10.4.1@v4.0)
  *   b200_gemm_fwd             torch.nn.Conv1d (strided, as GEMM),     bonito/nn.py:226,283-298,59-67
- *                             torch.nn.Linear + Clamp (LinearCRFEncoder), LSTM input projection
+ *                             torch.nn.Linear + Clamp (LinearCRFEncoder, the Linear in front of it), LSTM input projection
  *   b200_lstm_rec_fwd         koi.lstm.update_graph / torch.nn.LSTM   bonito/crf/model.py:240-246, bonito/nn.py:366-370
  *   b200_crf_decode           koi.decode.beam_search call contract    bonito/crf/basecall.py:36-40
  *                             with SeqdistModel.decode_batch maths    bonito/crf/model.py:98-108,196-199
+ *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
  *
  * Conventions (SURVEY.md section 8b): every function returns 0 on success and a negative value on
  * failure, with a message available from b200_last_error().  All pointers are raw DEVICE pointers
@@ -39,6 +41,9 @@ extern "C" {
  * as used by bonito/transformer/model.py:100-104.  n % 64 == 0, no bias. */
 #define B200_ACT_SWIGLU 5
 #define B200_ACT_TANH_SCALE 6 /* tanh, then multiply by lo: LinearCRFEncoder(activation="tanh", scale=5.0), bonito/nn.py:283-298 */
+/* swish, rounded to fp16, then clamp(lo, hi): a Convolution with activation "swish" followed by a Clamp layer
+ * (dna_r10.4.1@v4.0: Clamp(-0.5, 3.5) after each of the three convolutions) */
+#define B200_ACT_SWISH_CLAMP 7
 
 #define B200_GEMM_AUTO 0 /* the wgmma kernel (product path) unless B200_GEMM_IMPL=mma is set in the environment */
 #define B200_GEMM_TCGEN05 1 /* the wgmma kernel (the name is kept for ABI compatibility) */
@@ -60,6 +65,11 @@ const char* b200_last_error(void);
 int b200_conv_stem_fwd(const void* x, int n, int l, int c1, int k1, const void* w1, const void* b1, int act1,
                        int c2, int k2, const void* w2, const void* b2, int act2, void* out, int lp, int padl,
                        void* stream);
+/* Same, with the bounds (lo1, hi1) / (lo2, hi2) of act1 / act2 (used by B200_ACT_SWISH_CLAMP and B200_ACT_CLAMP; the entry
+ * point above passes zeros). */
+int b200_conv_stem_fwd_ex(const void* x, int n, int l, int c1, int k1, const void* w1, const void* b1, int act1, float lo1,
+                          float hi1, int c2, int k2, const void* w2, const void* b2, int act2, float lo2, float hi2, void* out,
+                          int lp, int padl, void* stream);
 
 /*
  * C = act(A[M,K] * B[N,K]^T + bias) in fp16 with fp32 accumulation.
@@ -192,6 +202,16 @@ size_t b200_crf_decode_workspace_bytes(int n, int t, int state_len);
  */
 int b200_crf_decode(const void* scores, int n, int t, int state_len, float blank_score, float qscale, float qbias,
                     void* workspace, void* moves, void* sequence, void* qstring, void* stream);
+
+/*
+ * The same decode for heads with LEARNED blank scores (LinearCRFEncoder without blank_score, e.g. dna_r9.4.1@v3):
+ *   scores [N][T][5 * 4^state_len] fp16, 16-byte aligned, in the CTC_CRF layout [state][stay, move 0..3]
+ *   (bonito/crf/model.py:37-42): the stay edge of state s at frame t scores scores[t][s*5], its in-edge 1+j scores[t][s*5+1+j].
+ * Same passes, arithmetic, tie-breaks, outputs and quality rule as b200_crf_decode; the workspace is the same size, so
+ * b200_crf_decode_workspace_bytes(n, t, state_len) covers it.
+ */
+int b200_crf_decode_lb(const void* scores, int n, int t, int state_len, float qscale, float qbias, void* workspace, void* moves,
+                       void* sequence, void* qstring, void* stream);
 
 /*
  * ---- chunk() on the device (reference: bonito.util.chunk, bonito/util.py:142-161) ----
