@@ -14,6 +14,7 @@ from time import perf_counter
 
 import numpy as np
 
+from bonito_b200.ctc.model import Model as CtcModel
 from bonito_b200.io import Writer, biofmt
 from bonito_b200.nn import fuse_bn_
 from bonito_b200.reader import Reader
@@ -51,6 +52,12 @@ def main(args):
         model = model.apply(fuse_bn_)
     except FileNotFoundError:
         sys.stderr.write(f"> error: failed to load {args.model_directory}\n")
+        exit(1)
+    except ImportError as err:                  # a model package this build does not have
+        sys.stderr.write(f"> error: no native path for this model (there is no eager fallback): {err}\n")
+        exit(1)
+    if args.revcomp and isinstance(model, CtcModel):
+        sys.stderr.write("> error: --revcomp is not supported for the QuartzNet CTC models (dna_r9.4.1@v1, @v2)\n")
         exit(1)
     try:
         # build the native plan now: a layer stack without a native kernel is reported here, not from the writer thread

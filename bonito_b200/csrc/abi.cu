@@ -14,6 +14,12 @@ int launch_lstm_rec(const __half* gx, const __half* whh, __half* y, int T, int N
                     cudaStream_t stream);
 int launch_conv_first(const __half* x, int N, int L, int C, int K, const __half* w, const __half* bias, int act,
                       __half* out, int Lp, int padl, cudaStream_t stream);
+int launch_conv_first_ex(const __half* x, int N, int L, int C, int K, int S, const __half* w, const __half* bias, int act,
+                         float lo, float hi, __half* out, long long ldo, int Lp, int padl, cudaStream_t stream);
+int launch_depthwise(const __half* x, long long ldx, const __half* w, __half* y, long long ldy, int N, int T, int C, int K,
+                     cudaStream_t stream);
+int launch_ctc_head(const __half* x, long long M, int F, const __half* w, const __half* bias, __half* logp, uint8_t* labels,
+                    float* probs, cudaStream_t stream);
 int launch_rmsnorm_residual(const __half* a, const __half* x, const __half* w, float alpha, float eps, __half* out,
                             long long M, int D, cudaStream_t stream);
 int launch_swiglu(const __half* h, __half* out, long long M, int F, cudaStream_t stream);
@@ -135,6 +141,34 @@ int b200_conv_first_fwd(const void* x, int n, int l, int c, int k, const void* w
     if (n == 0) return 0;
     return launch_conv_first((const __half*)x, n, l, c, k, (const __half*)w, (const __half*)bias, act, (__half*)out, lp,
                              padl, (cudaStream_t)stream);
+}
+
+int b200_conv_first_fwd_ex(const void* x, int n, int l, int c, int k, int stride, const void* w, const void* bias, int act,
+                           float lo, float hi, void* out, long long ldo, int lp, int padl, void* stream) {
+    B200_REQUIRE(x && w && out, "conv_first_ex: null pointer argument");
+    B200_REQUIRE(n >= 0 && l > 0 && lp > 0 && padl >= 0, "conv_first_ex: bad sizes n=%d l=%d lp=%d padl=%d", n, l, lp, padl);
+    if (n == 0) return 0;
+    B200_REQUIRE(n <= 65535, "conv_first_ex: at most 65535 chunks per call (n=%d)", n);
+    return launch_conv_first_ex((const __half*)x, n, l, c, k, stride, (const __half*)w, (const __half*)bias, act, lo, hi,
+                                (__half*)out, ldo, lp, padl, (cudaStream_t)stream);
+}
+
+int b200_depthwise_conv_fwd(const void* x, long long ldx, const void* w, void* y, long long ldy, int n, int t, int c, int k,
+                            void* stream) {
+    B200_REQUIRE(x && w && y, "depthwise: null pointer argument");
+    B200_REQUIRE(n >= 0 && t >= 0, "depthwise: bad sizes n=%d t=%d", n, t);
+    if (n == 0 || t == 0) return 0;
+    B200_REQUIRE(n <= 65535, "depthwise: at most 65535 chunks per call (n=%d)", n);
+    return launch_depthwise((const __half*)x, ldx, (const __half*)w, (__half*)y, ldy, n, t, c, k, (cudaStream_t)stream);
+}
+
+int b200_ctc_head_fwd(const void* x, long long m, int f, const void* w, const void* bias, void* logp, void* labels, void* probs,
+                      void* stream) {
+    B200_REQUIRE(x && w && labels && probs, "ctc_head: null pointer argument");
+    B200_REQUIRE(m >= 0, "ctc_head: bad row count %lld", m);
+    if (m == 0) return 0;
+    return launch_ctc_head((const __half*)x, m, f, (const __half*)w, (const __half*)bias, (__half*)logp, (uint8_t*)labels,
+                           (float*)probs, (cudaStream_t)stream);
 }
 
 int b200_attention_fwd(void* qkv, const void* cos_sin, void* out, int n, int t, int heads, int head_dim, int wl,

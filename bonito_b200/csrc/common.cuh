@@ -88,6 +88,7 @@ __device__ __forceinline__ float apply_act_f16(float v, int act, float lo, float
         case B200_ACT_SCALE: return round_f16(v * lo);
         case B200_ACT_TANH_SCALE: return round_f16(round_f16(tanh_f(v)) * lo);
         case B200_ACT_SWISH_CLAMP: return fminf(fmaxf(round_f16(swish_f(v)), lo), hi);
+        case B200_ACT_RELU: return fmaxf(v, 0.f);
         default: return v;
     }
 }

@@ -1,0 +1,236 @@
+"""
+QuartzNet CTC model package (`package = "bonito.ctc"`: dna_r9.4.1@v1 and @v2).
+
+`Model(config)` mirrors the reference's module tree (bonito/ctc/model.py: `Encoder`, `Block`, `TCSConv1d`, `Decoder`, with
+the same attribute names and registration order), so a reference `weights_N.tar` loads through `match_names` unchanged,
+BatchNorm running statistics included.  On the CPU without `use_koi` the module tree runs and returns `[T, N, 5]`
+log-probs, as the reference's `forward` does.  With `use_koi` the native engine (`bonito_b200.engine_ctc.CtcPlan`) runs
+it on the GPU and returns batch-first `[N, T, 5]` fp16 log-probs; there is no eager CUDA path.
+"""
+
+import numpy as np
+import torch
+from torch.nn import BatchNorm1d, Conv1d, Dropout, Module, ModuleList, Sequential
+from torch.nn.functional import log_softmax
+
+from bonito_b200.nn import Permute, layers
+
+
+class Model(Module):
+    """QuartzNet-style CTC model (reference: bonito/ctc/model.py:15-60)."""
+
+    def __init__(self, config):
+        super().__init__()
+        if "qscore" not in config:
+            self.qbias, self.qscale = 0.0, 1.0
+        else:
+            self.qbias, self.qscale = config["qscore"]["bias"], config["qscore"]["scale"]
+        self.config = config
+        self.stride = config["block"][0]["stride"][0]
+        self.alphabet = config["labels"]["labels"]
+        self.features = config["block"][-1]["filters"]
+        self.encoder = Encoder(config)
+        self.decoder = Decoder(self.features, len(self.alphabet))
+        self._native = None        # set by use_koi(): dict of basecaller settings
+        self._plan = None          # built lazily, after the weights are loaded
+
+    def forward(self, x):
+        """[N, 1, L] -> log-probs: [T, N, 5] from the module tree on the CPU, [N, T, 5] fp16 from the native engine."""
+        if self._native is None:
+            if x.is_cuda:
+                raise RuntimeError("bonito_b200: CUDA model called without use_koi(); call model.use_koi(...) "
+                                   "(load_model(..., use_koi=True)) or run the module tree on the CPU")
+            return self.decoder(self.encoder(x))
+        return self.native_plan(x.device if x.is_cuda else None).forward(x)
+
+    def native_plan(self, device=None):
+        from bonito_b200 import native
+        from bonito_b200.engine_ctc import CtcPlan
+        native.require()
+        if device is None:
+            device = next(self.parameters()).device
+        if torch.device(device).type != "cuda":
+            raise native.NativeError("the native path was requested (use_koi) but the model is not on a CUDA device")
+        if self._plan is None or self._plan.device != torch.device(device):
+            self._plan = CtcPlan(self, device, quantize=bool((self._native or {}).get("quantize")))
+        return self._plan
+
+    def invalidate_plan(self):
+        self._plan = None
+
+    def _apply(self, fn, *args, **kwargs):
+        self._plan = None  # .half()/.to() change the tensors the plan was packed from
+        return super()._apply(fn, *args, **kwargs)
+
+    def apply(self, fn):
+        self._plan = None
+        return super().apply(fn)
+
+    def load_state_dict(self, *args, **kwargs):
+        self._plan = None  # the plan holds folded copies of the weights
+        return super().load_state_dict(*args, **kwargs)
+
+    def use_koi(self, **kwargs):
+        """Arm the native engine (the hook `_load_model` calls)."""
+        self._native = dict(kwargs)
+        self._plan = None
+
+    def decode(self, x, beamsize=1, qscores=False, return_path=False):
+        """
+        Greedy CTC decode of one `[T, 5]` log-prob tensor (see `greedy_collapse`).  Returns the sequence, with the quality
+        string appended when `qscores` (the layout of the reference's viterbi_search), and the emission frames when
+        `return_path`.  The CTC prefix beam search (`beamsize > 1`) is not implemented.
+        """
+        if beamsize != 1:
+            raise NotImplementedError("CTC beam search is not implemented; use beamsize=1")
+        logp = x.detach().float().cpu().numpy()
+        labels, probs = greedy_step(logp)
+        seq, qstring, moves = greedy_collapse(labels, probs, self.alphabet, self.qscale, self.qbias)
+        seq = seq[seq != 0].tobytes().decode()
+        if qscores:
+            seq += qstring[qstring != 0].tobytes().decode()
+        if return_path:
+            return seq, np.flatnonzero(moves)
+        return seq
+
+
+def greedy_step(logp):
+    """Per-frame argmax of [..., 5] log-probs (equal values: the highest index wins) and its probability exp(logp)."""
+    logp = np.asarray(logp, dtype=np.float32)
+    labels = (logp.shape[-1] - 1 - np.argmax(logp[..., ::-1], axis=-1)).astype(np.uint8)
+    probs = np.exp(np.take_along_axis(logp, labels[..., None].astype(np.int64), axis=-1)[..., 0]).astype(np.float32)
+    return labels, probs
+
+
+def greedy_collapse(labels, probs, alphabet, qscale=1.0, qbias=0.0):
+    """
+    Greedy CTC collapse of one read's per-frame labels [T] (uint8, 0 = blank) and probabilities [T] (fp32):
+      * frame t emits a base when labels[t] != 0 and labels[t] != labels[t - 1] (frame -1 has no label; blanks reset, so
+        A _ A emits two A);
+      * the quality of a base is phred(mean of probs over the non-blank frames from its emission up to the next emission),
+        phred(p) = clip(rint(-10 log10(max(1 - p, 1e-4)) * qscale + qbias) + 33, 33, 126).
+    Returns (sequence, qstring, moves) as uint8 [T] arrays: the character / quality on emitting frames and 0 elsewhere,
+    moves 1 on emitting frames (the byte layout of the CRF decoder's outputs).
+    """
+    labels = np.asarray(labels, dtype=np.uint8)
+    probs = np.asarray(probs, dtype=np.float32)
+    T = labels.shape[0]
+    seq = np.zeros(T, dtype=np.uint8)
+    qual = np.zeros(T, dtype=np.uint8)
+    moves = np.zeros(T, dtype=np.uint8)
+    if T == 0:
+        return seq, qual, moves
+    prev = np.concatenate([[0], labels[:-1]]).astype(np.uint8)
+    emit = (labels != 0) & (labels != prev)
+    starts = np.flatnonzero(emit)
+    if starts.size == 0:
+        return seq, qual, moves
+    moves[starts] = 1
+    letters = np.frombuffer("".join(alphabet).encode(), dtype=np.uint8)
+    seq[starts] = letters[labels[starts]]
+    # run means over the non-blank frames of each emission's span [start_i, start_{i+1})
+    nonblank = (labels != 0).astype(np.float64)
+    sums = np.add.reduceat(probs.astype(np.float64) * nonblank, starts)
+    counts = np.add.reduceat(nonblank, starts)
+    mean = sums / counts
+    err = np.maximum(1.0 - mean, 1e-4)
+    q = np.rint(-10.0 * np.log10(err) * qscale + qbias) + 33
+    qual[starts] = np.clip(q, 33, 126).astype(np.uint8)
+    return seq, qual, moves
+
+
+class Encoder(Module):
+    """The blocks of a `[[block]]` config (reference: bonito/ctc/model.py:63-87)."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = config
+        features = self.config["input"]["features"]
+        activation = layers[self.config["encoder"]["activation"]]()
+        encoder_layers = []
+        for layer in self.config["block"]:
+            encoder_layers.append(Block(features, layer["filters"], activation, repeat=layer["repeat"],
+                                        kernel_size=layer["kernel"], stride=layer["stride"], dilation=layer["dilation"],
+                                        dropout=layer["dropout"], residual=layer["residual"], separable=layer["separable"]))
+            features = layer["filters"]
+        self.encoder = Sequential(*encoder_layers)
+
+    def forward(self, x):
+        return self.encoder(x)
+
+
+class TCSConv1d(Module):
+    """Time-channel separable Conv1d: depthwise then pointwise, or one dense Conv1d (reference: bonito/ctc/model.py:90-121)."""
+
+    def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, bias=False,
+                 separable=False):
+        super().__init__()
+        self.separable = separable
+        if separable:
+            self.depthwise = Conv1d(in_channels, in_channels, kernel_size=kernel_size, stride=stride, padding=padding,
+                                    dilation=dilation, bias=bias, groups=in_channels)
+            self.pointwise = Conv1d(in_channels, out_channels, kernel_size=1, stride=1, dilation=dilation, bias=bias,
+                                    padding=0)
+        else:
+            self.conv = Conv1d(in_channels, out_channels, kernel_size=kernel_size, stride=stride, padding=padding,
+                               dilation=dilation, bias=bias)
+
+    def forward(self, x):
+        if self.separable:
+            return self.pointwise(self.depthwise(x))
+        return self.conv(x)
+
+
+class Block(Module):
+    """repeat x [TCSConv1d, BatchNorm1d(eps=1e-3)] with activation + Dropout between repeats, the optional residual
+    [Conv1d 1x1, BatchNorm1d] of the block input added before the last activation (reference: bonito/ctc/model.py:124-192)."""
+
+    def __init__(self, in_channels, out_channels, activation, repeat=5, kernel_size=1, stride=1, dilation=1, dropout=0.0,
+                 residual=False, separable=False):
+        super().__init__()
+        self.use_res = residual
+        self.conv = ModuleList()
+        _in_channels = in_channels
+        padding = self.get_padding(kernel_size[0], stride[0], dilation[0])
+        for _ in range(repeat - 1):
+            self.conv.extend(self.get_tcs(_in_channels, out_channels, kernel_size=kernel_size, stride=stride,
+                                          dilation=dilation, padding=padding, separable=separable))
+            self.conv.extend(self.get_activation(activation, dropout))
+            _in_channels = out_channels
+        self.conv.extend(self.get_tcs(_in_channels, out_channels, kernel_size=kernel_size, stride=stride, dilation=dilation,
+                                      padding=padding, separable=separable))
+        if self.use_res:
+            self.residual = Sequential(*self.get_tcs(in_channels, out_channels))
+        self.activation = Sequential(*self.get_activation(activation, dropout))
+
+    def get_activation(self, activation, dropout):
+        return activation, Dropout(p=dropout)
+
+    def get_padding(self, kernel_size, stride, dilation):
+        if stride > 1 and dilation > 1:
+            raise ValueError("Dilation and stride can not both be greater than 1")
+        return (kernel_size // 2) * dilation
+
+    def get_tcs(self, in_channels, out_channels, kernel_size=1, stride=1, dilation=1, padding=0, bias=False, separable=False):
+        return [TCSConv1d(in_channels, out_channels, kernel_size, stride=stride, dilation=dilation, padding=padding, bias=bias,
+                          separable=separable),
+                BatchNorm1d(out_channels, eps=1e-3, momentum=0.1)]
+
+    def forward(self, x):
+        _x = x
+        for layer in self.conv:
+            _x = layer(_x)
+        if self.use_res:
+            _x = _x + self.residual(x)
+        return self.activation(_x)
+
+
+class Decoder(Module):
+    """Conv1d(features -> classes, k1, bias) -> Permute([2, 0, 1]) -> log_softmax (reference: bonito/ctc/model.py:195-208)."""
+
+    def __init__(self, features, classes):
+        super().__init__()
+        self.layers = Sequential(Conv1d(features, classes, kernel_size=1, bias=True), Permute([2, 0, 1]))
+
+    def forward(self, x):
+        return log_softmax(self.layers(x), dim=-1)

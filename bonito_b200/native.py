@@ -15,7 +15,7 @@ import torch
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libbonito_b200.so")
 _lib = None
 
-ACT_NONE, ACT_SWISH, ACT_TANH, ACT_CLAMP, ACT_SCALE, ACT_SWIGLU, ACT_TANH_SCALE, ACT_SWISH_CLAMP = 0, 1, 2, 3, 4, 5, 6, 7
+ACT_NONE, ACT_SWISH, ACT_TANH, ACT_CLAMP, ACT_SCALE, ACT_SWIGLU, ACT_TANH_SCALE, ACT_SWISH_CLAMP, ACT_RELU = 0, 1, 2, 3, 4, 5, 6, 7, 8
 GEMM_AUTO, GEMM_TCGEN05, GEMM_MMA_SYNC = 0, 1, 2
 
 MAX_LSTM_LAYERS = 8
@@ -51,6 +51,11 @@ SIGNATURES = {
                                  c_int, c_int, c_void_p]),
     "b200_conv_first_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                     c_int, c_void_p]),
+    "b200_conv_first_fwd_ex": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_float,
+                                       c_void_p, c_longlong, c_int, c_int, c_void_p]),
+    "b200_depthwise_conv_fwd": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_int,
+                                        c_void_p]),
+    "b200_ctc_head_fwd": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b200_rmsnorm_residual_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_void_p, c_longlong, c_int,
                                           c_void_p]),
@@ -189,6 +194,42 @@ def conv_first(x, w, bias, act, out, lp, padl, stream=None):
                                      padl, _stream(stream))
     _check(rc, "b200_conv_first_fwd")
     return out
+
+
+def conv_first_ex(x, w, bias, act, out, ldo, lp, padl, stride=1, lo=0.0, hi=0.0, stream=None):
+    """x [N,L] -> rows n*lp + padl + t (t < (L-1)//stride + 1) of `out`, pitch `ldo` elements (see b200_conv_first_fwd_ex);
+    `out` only supplies the base pointer, so it may be a column offset into a wider buffer."""
+    lib = require()
+    n, l = x.shape
+    c, _, k = w.shape
+    with torch.cuda.device(x.device):
+        rc = lib.b200_conv_first_fwd_ex(_ptr(_f16(x, "x")), n, l, c, k, int(stride), _ptr(_f16(w, "w")), _ptr(bias), act,
+                                        float(lo), float(hi), _ptr(out), int(ldo), lp, padl, _stream(stream))
+    _check(rc, "b200_conv_first_fwd_ex")
+    return out
+
+
+def depthwise_conv(x, ldx, w, y, ldy, n, t, stream=None):
+    """Depthwise Conv1d over n chunks of t channels-last rows (see b200_depthwise_conv_fwd); w [C, 1, K]; `x` / `y` only
+    supply base pointers (column ranges of wider buffers with pitches ldx / ldy)."""
+    lib = require()
+    c, _, k = w.shape
+    with torch.cuda.device(y.device):
+        rc = lib.b200_depthwise_conv_fwd(_ptr(x), int(ldx), _ptr(_f16(w, "w")), _ptr(y), int(ldy), int(n), int(t), c, k,
+                                         _stream(stream))
+    _check(rc, "b200_depthwise_conv_fwd")
+    return y
+
+
+def ctc_head(x, m, w, bias, labels, probs, logp=None, stream=None):
+    """x [m, F] -> labels uint8 [m], probs fp32 [m] and, when given, logp fp16 [m, 5] (see b200_ctc_head_fwd)."""
+    lib = require()
+    f = w.shape[-1]
+    with torch.cuda.device(labels.device):
+        rc = lib.b200_ctc_head_fwd(_ptr(_f16(x, "x")), int(m), f, _ptr(_f16(w, "w")), _ptr(bias), _ptr(logp), _ptr(labels),
+                                   _ptr(probs), _stream(stream))
+    _check(rc, "b200_ctc_head_fwd")
+    return labels, probs
 
 
 def attention(qkv, cos_sin, out, n, t, heads, head_dim, wl, wr, stream=None):

@@ -306,3 +306,105 @@ def sup_state_dict(spec, weights, prefix="encoder."):
     for l in range(spec["depth"]):
         sd[f"{prefix}transformer_encoder.{l}.deepnorm_alpha"] = torch.tensor(spec["alpha"])
     return sd
+
+
+# ---------------------------------------------------------------------------------------------------
+# QuartzNet CTC shapes: dna_r9.4.1@v1 / @v2 (bonito/models/configs/dna_r9.4.1@v1.toml, @v2.toml)
+# ---------------------------------------------------------------------------------------------------
+
+QUARTZNET = {
+    # name: (activation, [(filters, repeat, kernel, stride, residual, separable)] for C1, B1..B5, C2, C3)
+    "v1": ("relu", [(256, 1, 33, 3, False, False), (256, 5, 33, 1, True, True), (256, 5, 39, 1, True, True),
+                    (512, 5, 51, 1, True, True), (512, 5, 63, 1, True, True), (512, 5, 75, 1, True, True),
+                    (512, 1, 87, 1, False, True), (1024, 1, 1, 1, False, False)]),
+    "v2": ("swish", [(344, 1, 9, 3, False, False), (424, 2, 115, 1, True, True), (464, 7, 5, 1, True, True),
+                     (456, 4, 123, 1, True, True), (440, 9, 9, 1, True, True), (280, 6, 31, 1, True, True),
+                     (384, 1, 67, 1, False, True), (48, 1, 15, 1, False, False)]),
+}
+
+
+def quartznet_spec(name="v1", max_repeat=None):
+    """Shapes of dna_r9.4.1@v1 ("v1", relu) or @v2 ("v2", swish); `max_repeat` caps the repeats (reduced test variants)."""
+    activation, blocks = QUARTZNET[name]
+    if max_repeat is not None:
+        blocks = [(f, min(r, max_repeat), k, s, res, sep) for f, r, k, s, res, sep in blocks]
+    return dict(name=f"quartznet_{name}", activation=activation, blocks=list(blocks), stride=blocks[0][3])
+
+
+def quartznet_config(spec, batchsize=64, chunksize=4000, overlap=500, qscore=None):
+    """TOML-equivalent dict of a `[[block]]` config (`package = "bonito.ctc"`); `qscore=(scale, bias)` adds a [qscore]."""
+    cfg = {
+        "model": {"package": "bonito.ctc"},
+        "labels": {"labels": ["N", "A", "C", "G", "T"]},
+        "input": {"features": 1},
+        "encoder": {"activation": spec["activation"]},
+        "block": [dict(filters=f, repeat=r, kernel=[k], stride=[s], dilation=[1], dropout=0.0, residual=res, separable=sep)
+                  for f, r, k, s, res, sep in spec["blocks"]],
+        "basecaller": {"batchsize": batchsize, "chunksize": chunksize, "overlap": overlap},
+    }
+    if qscore is not None:
+        cfg["qscore"] = {"scale": float(qscore[0]), "bias": float(qscore[1])}
+    return cfg
+
+
+def make_quartznet_weights(spec, seed=25, conv_gain=0.5, head_gain=2.0):
+    """
+    Seeded fp16-representable state dict for `bonito_b200.ctc.model.Model(quartznet_config(spec))`, keyed by the module
+    tree's names (the reference's, so it loads there too).  Convolutions ~ N(0, gain^2 / fan_in); every BatchNorm has
+    gamma ~ U(0.6, 1.4), beta ~ N(0, 0.1^2), running_mean ~ N(0, 0.2^2) and running_var log-uniform over [0.05, 4], except
+    channel 0, whose var is 0.01 with gamma 0.3: there eps = 1e-3 against 1e-5 changes the BatchNorm scale by 5 %.
+    Depthwise convolutions have gain 1; pointwise, residual and dense ones `conv_gain`.  The random BatchNorm statistics
+    multiply the second moment by E[gamma^2 / var] ~ 4.7, so conv_gain = 0.5 keeps the per-block RMS of both stacks
+    between 0.3 and 1 through all 8 blocks (0.7 already grows it ~15x over the stack, 1.6 overflows).  The head is then
+    centred and scaled on a seeded calibration read: each class's logit gets mean 0 and standard deviation `head_gain`
+    over the frames, so the per-frame argmax moves between all five classes.
+    """
+    from bonito_b200.ctc.model import Model
+    model = Model(quartznet_config(spec))
+    gen = torch.Generator().manual_seed(seed)
+    out = {}
+    for name, t in model.state_dict().items():
+        shape = t.shape
+        if name.endswith("num_batches_tracked"):
+            v = torch.tensor(100, dtype=torch.long)
+        elif name.endswith("running_var"):
+            u = torch.rand(shape, generator=gen)
+            v = torch.exp(np.log(0.05) + u * (np.log(4.0) - np.log(0.05)))
+            v[0] = 0.01
+        elif name.endswith("running_mean"):
+            v = 0.2 * torch.randn(shape, generator=gen)
+        elif len(shape) == 1 and name.startswith("encoder") and name.endswith(".weight"):      # BatchNorm gamma
+            v = 0.6 + 0.8 * torch.rand(shape, generator=gen)
+            v[0] = 0.3
+        elif len(shape) == 1 and name.startswith("encoder") and name.endswith(".bias"):        # BatchNorm beta
+            v = 0.1 * torch.randn(shape, generator=gen)
+        elif name.startswith("decoder") and name.endswith(".bias"):
+            v = 0.1 * torch.randn(shape, generator=gen)
+        else:                                                                                  # Conv1d weight [out][in][k]
+            fan_in = shape[1] * shape[2]
+            gain = head_gain if name.startswith("decoder") else 1.0 if "depthwise" in name else conv_gain
+            v = torch.randn(shape, generator=gen) * (gain / np.sqrt(fan_in))
+        out[name] = v if v.dtype == torch.long else v.to(torch.float16).float()
+    # the encoder output has a large per-channel mean shared by every frame (relu / swish after random BatchNorm statistics),
+    # which would make one class win everywhere: centre and scale the head on a seeded calibration read instead
+    model.load_state_dict(out)
+    model.double().eval()          # float64: the calibrated fp16 head must not depend on the CPU's fp32 convolution paths
+    with torch.no_grad():
+        feats = model.encoder(squiggle(1, 900, seed=seed + 1).double())[0]          # [F, T]
+    w = out["decoder.layers.0.weight"][:, :, 0].double()
+    logits = w @ feats.double()
+    scale = head_gain / logits.std(dim=1, keepdim=True).clamp_min(1e-6)
+    w = w * scale
+    out["decoder.layers.0.weight"] = w[:, :, None].to(torch.float16).float()
+    out["decoder.layers.0.bias"] = (-(w @ feats.double()).mean(dim=1)).to(torch.float16).float()
+    return out
+
+
+def write_quartznet_dir(dirname, spec, state_dict, **config_kwargs):
+    """Write `config.toml` + `weights_1.tar` of a QuartzNet CTC model in the reference's format."""
+    import toml
+    os.makedirs(dirname, exist_ok=True)
+    with open(os.path.join(dirname, "config.toml"), "w") as fh:
+        toml.dump(quartznet_config(spec, **config_kwargs), fh)
+    torch.save(state_dict, os.path.join(dirname, "weights_1.tar"))
+    return dirname

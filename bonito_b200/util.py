@@ -37,6 +37,7 @@ __models_dir__ = __dir__ / "models"
 _PACKAGE_ALIASES = {
     "bonito.crf": "bonito_b200.crf",
     "bonito.transformer": "bonito_b200.transformer",
+    "bonito.ctc": "bonito_b200.ctc",
 }
 
 

@@ -9,6 +9,8 @@
  *   b200_gemm_fwd             torch.nn.Conv1d (strided, as GEMM),     bonito/nn.py:226,283-298,59-67
  *                             torch.nn.Linear + Clamp (LinearCRFEncoder, the Linear in front of it), LSTM input projection
  *   b200_lstm_rec_fwd         koi.lstm.update_graph / torch.nn.LSTM   bonito/crf/model.py:240-246, bonito/nn.py:366-370
+ *   b200_depthwise_conv_fwd   TCSConv1d.depthwise (QuartzNet CTC)      bonito/ctc/model.py:90-121
+ *   b200_ctc_head_fwd         Decoder + log_softmax, greedy argmax     bonito/ctc/model.py:195-208, ctc/basecall.py:53-58
  *   b200_crf_decode           koi.decode.beam_search call contract    bonito/crf/basecall.py:36-40
  *                             with SeqdistModel.decode_batch maths    bonito/crf/model.py:98-108,196-199
  *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
@@ -44,6 +46,7 @@ extern "C" {
 /* swish, rounded to fp16, then clamp(lo, hi): a Convolution with activation "swish" followed by a Clamp layer
  * (dna_r10.4.1@v4.0: Clamp(-0.5, 3.5) after each of the three convolutions) */
 #define B200_ACT_SWISH_CLAMP 7
+#define B200_ACT_RELU 8 /* max(x, 0): the QuartzNet CTC model dna_r9.4.1@v1 (bonito/ctc/model.py, [encoder] activation = "relu") */
 
 #define B200_GEMM_AUTO 0 /* the wgmma kernel (product path) unless B200_GEMM_IMPL=mma is set in the environment */
 #define B200_GEMM_TCGEN05 1 /* the wgmma kernel (the name is kept for ABI compatibility) */
@@ -172,6 +175,36 @@ int b200_lstm_rec_wide_fwd(const void* gx, const void* whh, void* y, void* works
  */
 int b200_conv_first_fwd(const void* x, int n, int l, int c, int k, const void* w, const void* bias, int act, void* out,
                         int lp, int padl, void* stream);
+
+/*
+ * Same for strided convolutions and wider outputs (the C1 block of the QuartzNet CTC models: 1 -> 256 k33 s3, 1 -> 344 k9 s3,
+ * BatchNorm folded into w / bias): T = (l - 1) / stride + 1 output frames (padding k/2), frame t of chunk n written to row
+ * n*lp + padl + t of `out` with row pitch `ldo` elements (so it can fill a column range of a wider buffer); the other rows
+ * of [n*lp, n*lp + lp) get zeros in the c columns.  lo / hi: bounds of B200_ACT_CLAMP / B200_ACT_SWISH_CLAMP.
+ * c % 8 == 0, c <= 512, odd k <= 33, 1 <= stride <= 8, ldo % 8 == 0, out 16-byte aligned.
+ */
+int b200_conv_first_fwd_ex(const void* x, int n, int l, int c, int k, int stride, const void* w, const void* bias, int act,
+                           float lo, float hi, void* out, long long ldo, int lp, int padl, void* stream);
+
+/*
+ * ---- QuartzNet CTC path: bonito/ctc/model.py ----
+ *
+ * Depthwise Conv1d (groups = channels, stride 1, padding k/2, no bias) on channels-last fp16 rows:
+ *   y[(n*t + i)*ldy + ch] = sum_j w[ch][j] * x[(n*t + i + j - k/2)*ldx + ch],  frames outside [0, t) of chunk n read as zero
+ * w [c][1][k] fp16 (torch layout).  fp32 accumulation, one rounding to fp16.  Supported: 256 <= c <= 512, c % 8 == 0,
+ * k in {5, 9, 31, 33, 39, 51, 63, 67, 75, 87, 115, 123}; ldx, ldy multiples of 8 and >= c, x 16-byte aligned.
+ */
+int b200_depthwise_conv_fwd(const void* x, long long ldx, const void* w, void* y, long long ldy, int n, int t, int c, int k,
+                            void* stream);
+
+/*
+ * CTC head + per-frame greedy step, for m rows of f features (x [m][f] fp16, f % 8 == 0, f <= 2048, 16-byte aligned):
+ *   logits = fp16(x w^T + bias)      w [5][f], bias [5] (may be NULL)
+ *   logp   = fp16(log_softmax(logits)) computed in fp32, written to logp [m][5] unless logp is NULL
+ *   labels [m] uint8 = argmax of logp (equal values: the highest index wins), probs [m] fp32 = exp(logp[label])
+ */
+int b200_ctc_head_fwd(const void* x, long long m, int f, const void* w, const void* bias, void* logp, void* labels, void* probs,
+                      void* stream);
 
 /*
  * Rotary embedding (NeoX half rotation, cos_sin [T][64] fp16 = cos[32] | sin[32] per position) + windowed softmax
