@@ -2,9 +2,9 @@
 from argparse import ArgumentParser, ArgumentDefaultsHelpFormatter
 
 from bonito_b200 import __version__
-from bonito_b200.cli import basecaller
+from bonito_b200.cli import basecaller, evaluate
 
-modules = ["basecaller"]
+modules = ["basecaller", "evaluate"]
 
 
 def main():
@@ -13,7 +13,7 @@ def main():
     subparsers = parser.add_subparsers(title="subcommands", description="valid commands", help="additional help",
                                        dest="command")
     subparsers.required = True
-    for name, mod in (("basecaller", basecaller),):
+    for name, mod in (("basecaller", basecaller), ("evaluate", evaluate)):
         p = subparsers.add_parser(name, parents=[mod.argparser()])
         p.set_defaults(func=mod.main)
     args = parser.parse_args()

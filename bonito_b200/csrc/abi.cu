@@ -20,6 +20,9 @@ int launch_depthwise(const __half* x, long long ldx, const __half* w, __half* y,
                      cudaStream_t stream);
 int launch_ctc_head(const __half* x, long long M, int F, const __half* w, const __half* bias, __half* logp, uint8_t* labels,
                     float* probs, cudaStream_t stream);
+size_t sw_align_workspace_bytes(int n_pairs, int max_ref_len);
+int launch_sw_align(const uint8_t* query, const long long* query_off, const int* query_len, const uint8_t* ref,
+                    const long long* ref_off, const int* ref_len, int n_pairs, void* workspace, int* out, cudaStream_t stream);
 int launch_rmsnorm_residual(const __half* a, const __half* x, const __half* w, float alpha, float eps, __half* out,
                             long long M, int D, cudaStream_t stream);
 int launch_swiglu(const __half* h, __half* out, long long M, int F, cudaStream_t stream);
@@ -169,6 +172,14 @@ int b200_ctc_head_fwd(const void* x, long long m, int f, const void* w, const vo
     if (m == 0) return 0;
     return launch_ctc_head((const __half*)x, m, f, (const __half*)w, (const __half*)bias, (__half*)logp, (uint8_t*)labels,
                            (float*)probs, (cudaStream_t)stream);
+}
+
+size_t b200_sw_align_workspace_bytes(int n_pairs, int max_ref_len) { return sw_align_workspace_bytes(n_pairs, max_ref_len); }
+
+int b200_sw_align(const void* query, const long long* query_off, const int* query_len, const void* ref, const long long* ref_off,
+                  const int* ref_len, int n_pairs, void* workspace, void* out, void* stream) {
+    return launch_sw_align((const uint8_t*)query, query_off, query_len, (const uint8_t*)ref, ref_off, ref_len, n_pairs,
+                           workspace, (int*)out, (cudaStream_t)stream);
 }
 
 int b200_attention_fwd(void* qkv, const void* cos_sin, void* out, int n, int t, int heads, int head_dim, int wl,

@@ -56,6 +56,8 @@ SIGNATURES = {
     "b200_depthwise_conv_fwd": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_int, c_int, c_int, c_int,
                                         c_void_p]),
     "b200_ctc_head_fwd": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_sw_align_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "b200_sw_align": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "b200_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b200_rmsnorm_residual_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_void_p, c_longlong, c_int,
                                           c_void_p]),
@@ -230,6 +232,33 @@ def ctc_head(x, m, w, bias, labels, probs, logp=None, stream=None):
                                    _ptr(probs), _stream(stream))
     _check(rc, "b200_ctc_head_fwd")
     return labels, probs
+
+
+def sw_align_workspace_bytes(n_pairs, max_ref_len):
+    return load().b200_sw_align_workspace_bytes(int(n_pairs), int(max_ref_len))
+
+
+def sw_align(query, query_off, query_len, ref, ref_off, ref_len, workspace, out, stream=None):
+    """Batched Smith-Waterman (see b200_sw_align): query / ref packed CUDA uint8 buffers; query_off / ref_off CPU int64 and
+    query_len / ref_len CPU int32 tensors of n_pairs entries; workspace CUDA uint8 of sw_align_workspace_bytes(n_pairs,
+    max(ref_len)) bytes; out CUDA int32 [n_pairs, 7]."""
+    lib = require()
+    n = query_len.numel()
+    for t, dtype, name in ((query_off, torch.int64, "query_off"), (ref_off, torch.int64, "ref_off"),
+                           (query_len, torch.int32, "query_len"), (ref_len, torch.int32, "ref_len")):
+        if t.is_cuda or t.dtype != dtype or not t.is_contiguous() or t.numel() != n:
+            raise NativeError(f"sw_align: {name} must be a contiguous host {dtype} tensor of {n} entries")
+    for t, dtype, name in ((query, torch.uint8, "query"), (ref, torch.uint8, "ref"), (workspace, torch.uint8, "workspace"),
+                           (out, torch.int32, "out")):
+        if not t.is_cuda or t.dtype != dtype or not t.is_contiguous():
+            raise NativeError(f"sw_align: {name} must be a contiguous CUDA {dtype} tensor")
+    if out.shape != (n, 7):
+        raise NativeError(f"sw_align: out must have shape ({n}, 7), got {tuple(out.shape)}")
+    with torch.cuda.device(out.device):
+        rc = lib.b200_sw_align(_ptr(query), _ptr(query_off), _ptr(query_len), _ptr(ref), _ptr(ref_off), _ptr(ref_len), n,
+                               _ptr(workspace), _ptr(out), _stream(stream))
+    _check(rc, "b200_sw_align")
+    return out
 
 
 def attention(qkv, cos_sin, out, n, t, heads, head_dim, wl, wr, stream=None):

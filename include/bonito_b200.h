@@ -11,6 +11,8 @@
  *   b200_lstm_rec_fwd         koi.lstm.update_graph / torch.nn.LSTM   bonito/crf/model.py:240-246, bonito/nn.py:366-370
  *   b200_depthwise_conv_fwd   TCSConv1d.depthwise (QuartzNet CTC)      bonito/ctc/model.py:90-121
  *   b200_ctc_head_fwd         Decoder + log_softmax, greedy argmax     bonito/ctc/model.py:195-208, ctc/basecall.py:53-58
+ *   b200_sw_align             parasail.sw_trace_striped_32 + CIGAR    bonito/cli/evaluate.py:37-67
+ *                             counts (`evaluate`)
  *   b200_crf_decode           koi.decode.beam_search call contract    bonito/crf/basecall.py:36-40
  *                             with SeqdistModel.decode_batch maths    bonito/crf/model.py:98-108,196-199
  *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
@@ -205,6 +207,21 @@ int b200_depthwise_conv_fwd(const void* x, long long ldx, const void* w, void* y
  */
 int b200_ctc_head_fwd(const void* x, long long m, int f, const void* w, const void* bias, void* logp, void* labels, void* probs,
                       void* stream);
+
+/*
+ * Batched Smith-Waterman local alignment with affine gaps (match +5, mismatch -4, gap open 8, extend 4; the tie rules are
+ * in bonito_b200/csrc/align.cu), for n_pairs pairs (query p, reference p) of ASCII A/C/G/T bytes.  `query` / `ref` are
+ * packed DEVICE byte buffers; pair p is query[query_off[p] .. + query_len[p]) against ref[ref_off[p] .. + ref_len[p]).
+ * Unlike the rest of this ABI, query_off / ref_off (int64) and query_len / ref_len (int32) are HOST arrays: the lengths
+ * are checked on the host (each in [0, 65535], else -2) and the four arrays are copied into the head of `workspace` on
+ * `stream`, so pinned arrays must stay unchanged until the stream has passed this call.  `workspace`: DEVICE memory of
+ * b200_sw_align_workspace_bytes(n_pairs, max_ref_len) bytes with max_ref_len >= every ref_len[p].
+ * out: int32 [n_pairs][7] = score, end_query, end_ref (0-based, inclusive), n_eq, n_x, n_ins, n_del of the traced
+ * alignment; a pair whose best score is 0 gives 0, -1, -1, 0, 0, 0, 0.  n_pairs == 0 is a no-op.
+ */
+size_t b200_sw_align_workspace_bytes(int n_pairs, int max_ref_len);
+int b200_sw_align(const void* query, const long long* query_off, const int* query_len, const void* ref, const long long* ref_off,
+                  const int* ref_len, int n_pairs, void* workspace, void* out, void* stream);
 
 /*
  * Rotary embedding (NeoX half rotation, cos_sin [T][64] fp16 = cos[32] | sin[32] per position) + windowed softmax
