@@ -23,6 +23,12 @@ int launch_ctc_head(const __half* x, long long M, int F, const __half* w, const 
 size_t sw_align_workspace_bytes(int n_pairs, int max_ref_len);
 int launch_sw_align(const uint8_t* query, const long long* query_off, const int* query_len, const uint8_t* ref,
                     const long long* ref_off, const int* ref_len, int n_pairs, void* workspace, int* out, cudaStream_t stream);
+size_t pair_align_trace_bytes(int mode, int m, int n, int band);
+size_t pair_align_workspace_bytes(int mode, int n_pairs, const int* query_len, const int* ref_len, const int* band,
+                                  int traceback);
+int launch_pair_align(int mode, const uint8_t* query, const long long* query_off, const int* query_len, const uint8_t* ref,
+                      const long long* ref_off, const int* ref_len, const int* band, int n_pairs, int traceback,
+                      void* workspace, uint8_t* ops, const long long* ops_off, int* out, cudaStream_t stream);
 int launch_rmsnorm_residual(const __half* a, const __half* x, const __half* w, float alpha, float eps, __half* out,
                             long long M, int D, cudaStream_t stream);
 int launch_swiglu(const __half* h, __half* out, long long M, int F, cudaStream_t stream);
@@ -180,6 +186,22 @@ int b200_sw_align(const void* query, const long long* query_off, const int* quer
                   const int* ref_len, int n_pairs, void* workspace, void* out, void* stream) {
     return launch_sw_align((const uint8_t*)query, query_off, query_len, (const uint8_t*)ref, ref_off, ref_len, n_pairs,
                            workspace, (int*)out, (cudaStream_t)stream);
+}
+
+size_t b200_pair_align_trace_bytes(int mode, int query_len, int ref_len, int band) {
+    return pair_align_trace_bytes(mode, query_len, ref_len, band);
+}
+
+size_t b200_pair_align_workspace_bytes(int mode, int n_pairs, const int* query_len, const int* ref_len, const int* band,
+                                       int traceback) {
+    return pair_align_workspace_bytes(mode, n_pairs, query_len, ref_len, band, traceback);
+}
+
+int b200_pair_align(int mode, const void* query, const long long* query_off, const int* query_len, const void* ref,
+                    const long long* ref_off, const int* ref_len, const int* band, int n_pairs, int traceback, void* workspace,
+                    void* ops, const long long* ops_off, void* out, void* stream) {
+    return launch_pair_align(mode, (const uint8_t*)query, query_off, query_len, (const uint8_t*)ref, ref_off, ref_len, band,
+                             n_pairs, traceback, workspace, (uint8_t*)ops, ops_off, (int*)out, (cudaStream_t)stream);
 }
 
 int b200_attention_fwd(void* qkv, const void* cos_sin, void* out, int n, int t, int heads, int head_dim, int wl,

@@ -101,6 +101,42 @@ def read_tags(read, res, group_key=None, with_moves=True):
     return tags
 
 
+class DuplexWriter(Thread):
+    """
+    Writes `duplex` consensus reads, named `<template id>;<complement id>` with a `qs:i:` tag (reference: bonito/io.py:472-502):
+    `iterator` yields ((template id, complement id), {"sequence", "qstring"}).  `.log` holds (read name, bases) of every
+    pair, written or not, as the reference counts them; empty and below-`min_qscore` consensuses are not written.
+    """
+
+    def __init__(self, iterator, fd=sys.stdout, min_qscore=0, mode="wfq"):
+        super().__init__(daemon=True)
+        if mode not in ("wfq", "w"):
+            raise ValueError(f"output mode {mode!r} needs htslib (BAM / CRAM), which this build does not bundle: "
+                             "redirect to a .sam or .fastq file")
+        self.iterator, self.fd, self.min_qscore, self.mode = iterator, fd, min_qscore, mode
+        self.log, self.error = [], None
+
+    def run(self):
+        try:
+            if self.mode == "w":
+                self.fd.write(sam_header())
+            for (temp_id, comp_id), res in self.iterator:
+                read_id = f"{temp_id};{comp_id}"
+                seq, qstring = res["sequence"], res["qstring"]
+                mean_q = mean_qscore_from_qstring(qstring)
+                self.log.append((read_id, len(seq)))
+                if mean_q < self.min_qscore or not len(seq):
+                    continue
+                tags = [f"qs:i:{round(mean_q)}"]
+                if self.mode == "w":
+                    self.fd.write(sam_record(read_id, seq, qstring, tags=tags) + "\n")
+                else:
+                    write_fastq(read_id, seq, qstring, fd=self.fd, tags=tags)
+            self.fd.flush()
+        except BaseException as err:   # surfaced by the CLI after join()
+            self.error = err
+
+
 class Writer(Thread):
     """
     Drains the basecall iterator on its own thread; `.log` holds (read_id, num_samples) of the reads written.

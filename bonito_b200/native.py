@@ -10,6 +10,7 @@ import ctypes
 import os
 from ctypes import c_char_p, c_float, c_int, c_longlong, c_size_t, c_void_p
 
+import numpy as np
 import torch
 
 _LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "libbonito_b200.so")
@@ -58,6 +59,10 @@ SIGNATURES = {
     "b200_ctc_head_fwd": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_sw_align_workspace_bytes": (c_size_t, [c_int, c_int]),
     "b200_sw_align": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "b200_pair_align_trace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b200_pair_align_workspace_bytes": (c_size_t, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int]),
+    "b200_pair_align": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b200_rmsnorm_residual_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_float, c_void_p, c_longlong, c_int,
                                           c_void_p]),
@@ -258,6 +263,61 @@ def sw_align(query, query_off, query_len, ref, ref_off, ref_len, workspace, out,
         rc = lib.b200_sw_align(_ptr(query), _ptr(query_off), _ptr(query_len), _ptr(ref), _ptr(ref_off), _ptr(ref_len), n,
                                _ptr(workspace), _ptr(out), _stream(stream))
     _check(rc, "b200_sw_align")
+    return out
+
+
+PAIR_GLOBAL_EDIT, PAIR_SEMIGLOBAL_AFFINE = 0, 1
+
+
+def _host_i32(a, n, name):
+    """A contiguous int32 numpy copy of `n` entries (the per-pair host arrays of b200_pair_align)."""
+    a = np.ascontiguousarray(a, dtype=np.int32)
+    if a.shape != (n,):
+        raise NativeError(f"pair_align: {name} must have {n} entries, got shape {a.shape}")
+    return a
+
+
+def pair_align_trace_bytes(mode, query_len, ref_len, band=0):
+    return load().b200_pair_align_trace_bytes(int(mode), int(query_len), int(ref_len), int(band))
+
+
+def pair_align_workspace_bytes(mode, query_len, ref_len, band=None, traceback=True):
+    n = len(query_len)
+    ql, rl = _host_i32(query_len, n, "query_len"), _host_i32(ref_len, n, "ref_len")
+    bd = None if band is None else _host_i32(band, n, "band")
+    return load().b200_pair_align_workspace_bytes(int(mode), n, ql.ctypes.data, rl.ctypes.data,
+                                                  None if bd is None else bd.ctypes.data, int(bool(traceback)))
+
+
+def pair_align(mode, query, query_off, query_len, ref, ref_off, ref_len, band, workspace, out, ops=None, ops_off=None,
+               traceback=True, stream=None):
+    """Batched banded edit / semi-global affine alignment (see b200_pair_align): query / ref / ops / workspace CUDA uint8
+    buffers, out CUDA int32 [n, 2]; query_off / ref_off / ops_off int64 and query_len / ref_len / band int32 host numpy
+    arrays (copied into the workspace on `stream` before this returns)."""
+    lib = require()
+    n = len(query_len)
+    q_off, r_off = (np.ascontiguousarray(a, dtype=np.int64) for a in (query_off, ref_off))
+    ql, rl = _host_i32(query_len, n, "query_len"), _host_i32(ref_len, n, "ref_len")
+    bd = None if band is None else _host_i32(band, n, "band")
+    o_off = None if ops_off is None else np.ascontiguousarray(ops_off, dtype=np.int64)
+    for a, name in ((q_off, "query_off"), (r_off, "ref_off"), (o_off, "ops_off")):
+        if a is not None and a.shape != (n,):
+            raise NativeError(f"pair_align: {name} must have {n} entries")
+    for t, dtype, name in ((query, torch.uint8, "query"), (ref, torch.uint8, "ref"), (workspace, torch.uint8, "workspace"),
+                           (out, torch.int32, "out"), (ops, torch.uint8, "ops")):
+        if t is not None and (not t.is_cuda or t.dtype != dtype or not t.is_contiguous()):
+            raise NativeError(f"pair_align: {name} must be a contiguous CUDA {dtype} tensor")
+    if out.shape != (n, 2):
+        raise NativeError(f"pair_align: out must have shape ({n}, 2), got {tuple(out.shape)}")
+    need = pair_align_workspace_bytes(mode, ql, rl, bd, traceback)
+    if workspace.numel() < need:
+        raise NativeError(f"pair_align: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(out.device):
+        rc = lib.b200_pair_align(int(mode), _ptr(query), q_off.ctypes.data, ql.ctypes.data, _ptr(ref), r_off.ctypes.data,
+                                 rl.ctypes.data, None if bd is None else bd.ctypes.data, n, int(bool(traceback)),
+                                 _ptr(workspace), _ptr(ops), None if o_off is None else o_off.ctypes.data, _ptr(out),
+                                 _stream(stream))
+    _check(rc, "b200_pair_align")
     return out
 
 

@@ -13,6 +13,8 @@
  *   b200_ctc_head_fwd         Decoder + log_softmax, greedy argmax     bonito/ctc/model.py:195-208, ctc/basecall.py:53-58
  *   b200_sw_align             parasail.sw_trace_striped_32 + CIGAR    bonito/cli/evaluate.py:37-67
  *                             counts (`evaluate`)
+ *   b200_pair_align           edlib.align(task="path") and            bonito/cli/duplex.py:225-273
+ *                             parasail.sg_trace_scan_32 (`duplex`)
  *   b200_crf_decode           koi.decode.beam_search call contract    bonito/crf/basecall.py:36-40
  *                             with SeqdistModel.decode_batch maths    bonito/crf/model.py:98-108,196-199
  *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
@@ -222,6 +224,32 @@ int b200_ctc_head_fwd(const void* x, long long m, int f, const void* w, const vo
 size_t b200_sw_align_workspace_bytes(int n_pairs, int max_ref_len);
 int b200_sw_align(const void* query, const long long* query_off, const int* query_len, const void* ref, const long long* ref_off,
                   const int* ref_len, int n_pairs, void* workspace, void* out, void* stream);
+
+/*
+ * Batched pairwise alignment with a traceback, for `duplex` (the reference aligns with edlib.align(task="path") and
+ * parasail.sg_trace_scan_32; the scoring, band and tie rules here are this library's, in bonito_b200/csrc/pair_align.cu):
+ *   B200_PAIR_GLOBAL_EDIT        unit-cost global alignment restricted to the diagonals
+ *                                [min(0, n-m) - band[p], max(0, n-m) + band[p]]; the result is the unbanded optimum
+ *                                whenever the returned distance is <= band[p] (or band[p] >= max(m, n))
+ *   B200_PAIR_SEMIGLOBAL_AFFINE  match +5, mismatch -4, gap 10 + 2 (g - 1), free end gaps, full matrix
+ * Pair p is query[query_off[p] .. + query_len[p]) (rows, 'I' consumes it) against ref[ref_off[p] .. + ref_len[p])
+ * (columns, 'D' consumes it); `query` / `ref` are DEVICE byte buffers (equal bytes match).  As for b200_sw_align the
+ * per-pair arrays query_off, query_len, ref_off, ref_len, band (int32, GLOBAL_EDIT only, >= 0; values above max(m, n) act
+ * as max(m, n)) and ops_off (int64) are HOST arrays, checked on the host (lengths in [0, 2^28], else -2) and copied into
+ * the head of `workspace`.  workspace: DEVICE memory of b200_pair_align_workspace_bytes() bytes for the same arguments;
+ * b200_pair_align_trace_bytes() is the share of one pair (its traceback bits).
+ * traceback == 0 (GLOBAL_EDIT only): out[p][0] = the banded distance, nothing else is written and no trace bytes are needed.
+ * traceback != 0: out int32 [n_pairs][2] = score (distance / affine score), n_ops; the ops, one byte each of '=', 'X',
+ * 'I', 'D' in forward order, are the LAST n_ops bytes of the slot ops[ops_off[p] .. + query_len[p] + ref_len[p]) (DEVICE).
+ */
+#define B200_PAIR_GLOBAL_EDIT 0
+#define B200_PAIR_SEMIGLOBAL_AFFINE 1
+size_t b200_pair_align_trace_bytes(int mode, int query_len, int ref_len, int band);
+size_t b200_pair_align_workspace_bytes(int mode, int n_pairs, const int* query_len, const int* ref_len, const int* band,
+                                       int traceback);
+int b200_pair_align(int mode, const void* query, const long long* query_off, const int* query_len, const void* ref,
+                    const long long* ref_off, const int* ref_len, const int* band, int n_pairs, int traceback, void* workspace,
+                    void* ops, const long long* ops_off, void* out, void* stream);
 
 /*
  * Rotary embedding (NeoX half rotation, cos_sin [T][64] fp16 = cos[32] | sin[32] per position) + windowed softmax
