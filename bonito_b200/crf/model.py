@@ -2,14 +2,19 @@
 CTC-CRF model package (`Model`, `basecall` are what `load_symbol` looks up:
 `bonito/util.py:223-234`, `bonito/cli/basecaller.py:71`).
 
-Inference-only mirror of `bonito/crf/model.py`: the state graph (`CTC_CRF`),
-`SeqdistModel` and `Model` with the `use_koi` swap-in hook.  Training losses (koi.ctc) are out
-of scope (SURVEY.md section 2a row 12).
+Mirror of `bonito/crf/model.py`: the sequence distribution `CTC_CRF` with its scoring API and CTC
+loss (logZ, normalise, forward / backward scores, posteriors, viterbi, ctc_loss, ctc_viterbi_alignments:
+the koi.ctc calls of bonito/crf/model.py:47-143, here on the sm_90a kernels of csrc/ctc_crf.cu),
+`SeqdistModel` with `loss`, and `Model` with the `use_koi` swap-in hook.  The scoring API takes
+reference-layout scores [T, N, n_score()] on a CUDA device; gradients flow through autograd.
 """
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
+from bonito_b200.crf.lattice import Log, Max, sparse_backward_scores, sparse_forward_scores, sparse_logz, \
+    target_logz, target_viterbi
 from bonito_b200.nn import (Module, Convolution, LinearCRFEncoder, Serial, Permute, layers, to_dict, from_dict,
                             register)
 
@@ -61,6 +66,73 @@ class CTC_CRF:
     def path_to_str(self, path):
         letters = np.frombuffer("".join(self.alphabet).encode(), dtype="u1")
         return letters[path[path != 0]].tobytes().decode()
+
+    # -- scoring API (reference: bonito/crf/model.py:47-82, 98-103, 110-143) ------------------------------------------
+    # scores: [T, N, n_score()] on a CUDA device, the edge from idx[s, e] into s at column s*5 + e; fp16 is upcast to fp32
+    def logZ(self, scores, S=Log):
+        """logZ [N] of the whole lattice (alpha_0 = beta_T = S.one for every state)."""
+        return sparse_logz(scores, self.state_len, S)
+
+    def normalise(self, scores):
+        return scores - self.logZ(scores)[:, None] / len(scores)
+
+    def forward_scores(self, scores, S=Log):
+        """alpha [T+1, N, 4**state_len]."""
+        return sparse_forward_scores(scores, self.state_len, S)
+
+    def backward_scores(self, scores, S=Log):
+        """beta [T+1, N, 4**state_len]."""
+        return sparse_backward_scores(scores, self.state_len, S)
+
+    def compute_transition_probs(self, scores, betas):
+        T, N, C = scores.shape
+        log_trans = scores.reshape(T, N, -1, self.n_base + 1) + betas[1:, :, :, None]
+        # (new state, dropped base) -> (old state, emitted base)
+        log_trans = torch.cat([log_trans[:, :, :, [0]],
+                               log_trans[:, :, :, 1:].transpose(3, 2).reshape(T, N, -1, self.n_base)], dim=-1)
+        return torch.softmax(log_trans, dim=-1), torch.softmax(betas[0], dim=-1)
+
+    def posteriors(self, scores, S=Log):
+        """d logZ(scores, S).sum() / d scores, [T, N, n_score()]: edge marginals (Log) or the best path's one-hot (Max)."""
+        with torch.enable_grad():
+            x = scores.detach().requires_grad_()
+            grad, = torch.autograd.grad(self.logZ(x, S).sum(), x)
+        return grad
+
+    def viterbi(self, scores):
+        """Best path [T, N]: 0 on a stay, else 1 + the emitted base."""
+        a = self.posteriors(scores, Max).argmax(2)
+        moves = (a % len(self.alphabet)) != 0
+        return torch.where(moves, 1 + torch.div(a, len(self.alphabet), rounding_mode="floor") % self.n_base, 0)
+
+    def prepare_ctc_scores(self, scores, targets):
+        """Stay and move scores [T, N, L] / [T, N, L-1] of the k-mers along zero-padded targets [N, max_len] (1 + base)."""
+        targets = torch.clamp(targets - 1, 0)          # CTC labels (blank = 0) -> bases
+        T, N, C = scores.shape
+        scores = scores.to(torch.float32)
+        n = targets.size(1) - (self.state_len - 1)
+        stay_idx = sum(targets[:, i:n + i] * self.n_base ** (self.state_len - i - 1)
+                       for i in range(self.state_len)) * len(self.alphabet)
+        move_idx = stay_idx[:, 1:] + targets[:, :n - 1] + 1
+        return scores.gather(2, stay_idx.expand(T, -1, -1)), scores.gather(2, move_idx.expand(T, -1, -1))
+
+    def ctc_loss(self, scores, targets, target_lengths, loss_clip=None, reduction="mean", normalise_scores=True):
+        if reduction not in ("mean", "none", None):
+            raise ValueError("Unknown reduction type {}".format(reduction))
+        if normalise_scores:
+            scores = self.normalise(scores)
+        stay, move = self.prepare_ctc_scores(scores, targets)
+        logz = target_logz(stay, move, target_lengths + 1 - self.state_len)
+        loss = -(logz / target_lengths)
+        if loss_clip:
+            loss = torch.clamp(loss, 0.0, loss_clip)
+        return loss.mean() if reduction == "mean" else loss
+
+    def ctc_viterbi_alignments(self, scores, targets, target_lengths):
+        """One-hot [T, N, L] of the best alignment: a stay at j and the move j -> j+1 both mark column j."""
+        stay, move = self.prepare_ctc_scores(scores, targets)
+        dstay, dmove = target_viterbi(stay, move, target_lengths + 1 - self.state_len)
+        return dstay + F.pad(dmove, (0, 1))
 
 
 def conv(c_in, c_out, ks, stride=1, bias=False, activation=None, norm=None):
@@ -180,6 +252,12 @@ class SeqdistModel(Module):
 
     def decode(self, x):
         return self.decode_batch(x.unsqueeze(0))[0]
+
+    def loss(self, scores, targets, target_lengths, **kwargs):
+        """CTC-CRF loss of reference-layout scores [T, N, n_score()] (reference: bonito/crf/model.py:204-207)."""
+        if self.target_projection is not None:
+            targets = self.target_projection[targets]
+        return self.seqdist.ctc_loss(scores.to(torch.float32), targets, target_lengths, **kwargs)
 
     def _blank_score(self):
         """The head's fixed blank score; None when the head learns its blank scores (blank_score=None)."""

@@ -59,6 +59,20 @@ int launch_crf_beam_search(const __half* scores, int N, int T, int state_len, fl
 
 int launch_lstm_crf_fwd(const b200_lstm_crf_plan* p, const __half* x, __half* scores, cudaStream_t stream);
 
+size_t ctc_crf_sparse_workspace_bytes(int N, int T, int state_len, int semiring);
+size_t ctc_crf_target_workspace_bytes(int N, int T, int L, int semiring);
+int ctc_crf_target_max_states();
+int launch_ctc_crf_sparse_fwd(const float* scores, int T, int N, int state_len, int semiring, float* logz, float* alpha,
+                              void* workspace, cudaStream_t stream);
+int launch_ctc_crf_sparse_bwd(const float* scores, int T, int N, int state_len, int semiring, float* beta,
+                              cudaStream_t stream);
+int launch_ctc_crf_sparse_grad(const float* scores, int T, int N, int state_len, int semiring, const float* g,
+                               void* workspace, float* grad, cudaStream_t stream);
+int launch_ctc_crf_target_fwd(const float* stay, const float* move, const int* lengths, int T, int N, int L, int semiring,
+                              float* logz, void* workspace, cudaStream_t stream);
+int launch_ctc_crf_target_grad(const float* stay, const float* move, const int* lengths, int T, int N, int L, int semiring,
+                               const float* g, void* workspace, float* dstay, float* dmove, cudaStream_t stream);
+
 int launch_quantize_i8(const __half* x, int8_t* out, long long n, float scale, cudaStream_t stream);
 int launch_gemm_i8(const int8_t* A, long long lda, const int8_t* B, const float* col_scale, __half* C, long long ldc, int M,
                    int N, int K, const GemmEpilogue& ep, int max_ctas, cudaStream_t stream);
@@ -351,6 +365,72 @@ int b200_crf_beam_search(const void* scores, int n, int t, int state_len, float 
     B200_REQUIRE(scores && workspace && moves && sequence && qstring, "beam_search: null pointer argument");
     return launch_crf_beam_search((const __half*)scores, n, t, state_len, blank_score, beam_width, beam_cut, qscale, qbias,
                                   workspace, (uint8_t*)moves, (uint8_t*)sequence, (uint8_t*)qstring, (cudaStream_t)stream);
+}
+
+size_t b200_ctc_crf_sparse_workspace_bytes(int n, int t, int state_len, int semiring) {
+    if (n < 0 || t < 0 || state_len < 1 || state_len > 5) return 0;
+    return ctc_crf_sparse_workspace_bytes(n, t, state_len, semiring);
+}
+
+#define CTC_CRF_CHECK_SPARSE(what)                                                                                      \
+    B200_REQUIRE(n >= 0 && t >= 1, what ": bad sizes n=%d t=%d", n, t);                                                 \
+    B200_REQUIRE(semiring == B200_SEMIRING_LOG || semiring == B200_SEMIRING_MAX, what ": unknown semiring %d", semiring); \
+    B200_REQUIRE(scores && ((uintptr_t)scores & 15) == 0, what ": scores must be a 16-byte aligned device pointer")
+
+int b200_ctc_crf_sparse_fwd(const void* scores, int t, int n, int state_len, int semiring, void* logz, void* alpha,
+                            void* workspace, void* stream) {
+    CTC_CRF_CHECK_SPARSE("ctc_crf_sparse_fwd");
+    B200_REQUIRE(logz, "ctc_crf_sparse_fwd: null logz");
+    if (n == 0) return 0;
+    return launch_ctc_crf_sparse_fwd((const float*)scores, t, n, state_len, semiring, (float*)logz, (float*)alpha, workspace,
+                                     (cudaStream_t)stream);
+}
+
+int b200_ctc_crf_sparse_bwd(const void* scores, int t, int n, int state_len, int semiring, void* beta, void* stream) {
+    CTC_CRF_CHECK_SPARSE("ctc_crf_sparse_bwd");
+    B200_REQUIRE(beta, "ctc_crf_sparse_bwd: null beta");
+    if (n == 0) return 0;
+    return launch_ctc_crf_sparse_bwd((const float*)scores, t, n, state_len, semiring, (float*)beta, (cudaStream_t)stream);
+}
+
+int b200_ctc_crf_sparse_grad(const void* scores, int t, int n, int state_len, int semiring, const void* g, void* workspace,
+                             void* grad, void* stream) {
+    CTC_CRF_CHECK_SPARSE("ctc_crf_sparse_grad");
+    B200_REQUIRE(g && workspace && grad, "ctc_crf_sparse_grad: null pointer argument");
+    if (n == 0) return 0;
+    return launch_ctc_crf_sparse_grad((const float*)scores, t, n, state_len, semiring, (const float*)g, workspace,
+                                      (float*)grad, (cudaStream_t)stream);
+}
+
+int b200_ctc_crf_target_max_states(void) { return ctc_crf_target_max_states(); }
+
+size_t b200_ctc_crf_target_workspace_bytes(int n, int t, int l, int semiring) {
+    if (n < 0 || t < 0 || l < 1) return 0;
+    return ctc_crf_target_workspace_bytes(n, t, l, semiring);
+}
+
+#define CTC_CRF_CHECK_TARGET(what)                                                                                      \
+    B200_REQUIRE(n >= 0 && t >= 1 && l >= 1 && l <= ctc_crf_target_max_states(),                                        \
+                 what ": bad sizes n=%d t=%d l=%d (1 <= l <= %d)", n, t, l, ctc_crf_target_max_states());              \
+    B200_REQUIRE(semiring == B200_SEMIRING_LOG || semiring == B200_SEMIRING_MAX, what ": unknown semiring %d", semiring); \
+    B200_REQUIRE(stay && lengths && (move || l == 1), what ": null pointer argument")
+
+int b200_ctc_crf_target_fwd(const void* stay, const void* move, const void* lengths, int t, int n, int l, int semiring,
+                            void* logz, void* workspace, void* stream) {
+    CTC_CRF_CHECK_TARGET("ctc_crf_target_fwd");
+    B200_REQUIRE(logz, "ctc_crf_target_fwd: null logz");
+    if (n == 0) return 0;
+    return launch_ctc_crf_target_fwd((const float*)stay, (const float*)move, (const int*)lengths, t, n, l, semiring,
+                                     (float*)logz, workspace, (cudaStream_t)stream);
+}
+
+int b200_ctc_crf_target_grad(const void* stay, const void* move, const void* lengths, int t, int n, int l, int semiring,
+                             const void* g, void* workspace, void* dstay, void* dmove, void* stream) {
+    CTC_CRF_CHECK_TARGET("ctc_crf_target_grad");
+    B200_REQUIRE(g && workspace && dstay && (dmove || l == 1), "ctc_crf_target_grad: null pointer argument");
+    if (n == 0) return 0;
+    return launch_ctc_crf_target_grad((const float*)stay, (const float*)move, (const int*)lengths, t, n, l, semiring,
+                                      (const float*)g, workspace, (float*)dstay, (float*)dmove, (cudaStream_t)stream);
 }
 
 }  // extern "C"

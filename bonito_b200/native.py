@@ -94,6 +94,16 @@ SIGNATURES = {
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_crf_decode_lb": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float,
                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_crf_sparse_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b200_ctc_crf_sparse_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_crf_sparse_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b200_ctc_crf_sparse_grad": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_crf_target_max_states": (c_int, []),
+    "b200_ctc_crf_target_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b200_ctc_crf_target_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                        c_void_p]),
+    "b200_ctc_crf_target_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                         c_void_p, c_void_p, c_void_p]),
 }
 
 
@@ -463,6 +473,148 @@ def crf_beam_search(scores, state_len, blank_score, beam_width, beam_cut, qscale
                                       _ptr(qstring), _stream(stream))
     _check(rc, "b200_crf_beam_search")
     return moves, sequence, qstring
+
+
+SEMIRING_LOG, SEMIRING_MAX = 0, 1
+
+
+def _dev(t, dtype, name, what, shape=None):
+    """A contiguous CUDA tensor of `dtype` (and `shape`), or NativeError."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != dtype or not t.is_contiguous():
+        got = f"{t.dtype} {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+        raise NativeError(f"{what}: {name} must be a contiguous CUDA {dtype} tensor, got {got}")
+    if shape is not None and tuple(t.shape) != tuple(shape):
+        raise NativeError(f"{what}: {name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
+    return t
+
+
+def _semiring(semiring, what):
+    if semiring not in (SEMIRING_LOG, SEMIRING_MAX):
+        raise NativeError(f"{what}: unknown semiring {semiring!r}")
+    return semiring
+
+
+def _sparse_shape(scores, state_len, what):
+    _dev(scores, torch.float32, "scores", what)
+    if scores.dim() != 3 or scores.shape[2] != 5 * 4 ** state_len:
+        raise NativeError(f"{what}: scores must be [T, N, {5 * 4 ** state_len}] for state_len {state_len}, "
+                          f"got {tuple(scores.shape)}")
+    if scores.data_ptr() % 16:
+        raise NativeError(f"{what}: scores must be 16-byte aligned")
+    t, n, _ = scores.shape
+    return t, n
+
+
+def ctc_crf_sparse_workspace_bytes(n, t, state_len, semiring):
+    return load().b200_ctc_crf_sparse_workspace_bytes(int(n), int(t), int(state_len), int(semiring))
+
+
+def ctc_crf_sparse_fwd(scores, state_len, semiring, logz, alpha=None, workspace=None, stream=None):
+    """k-mer lattice forward (see b200_ctc_crf_sparse_fwd): scores [T, N, 5*4**state_len] fp32 -> logz [N]; alpha
+    [T+1, N, S] when given; `workspace` (uint8, ctc_crf_sparse_workspace_bytes bytes) keeps what ctc_crf_sparse_grad needs."""
+    lib = require()
+    what = "ctc_crf_sparse_fwd"
+    t, n = _sparse_shape(scores, state_len, what)
+    _dev(logz, torch.float32, "logz", what, (n,))
+    if alpha is not None:
+        _dev(alpha, torch.float32, "alpha", what, (t + 1, n, 4 ** state_len))
+    if workspace is not None:
+        _dev(workspace, torch.uint8, "workspace", what)
+        need = ctc_crf_sparse_workspace_bytes(n, t, state_len, semiring)
+        if workspace.numel() < need:
+            raise NativeError(f"{what}: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(scores.device):
+        rc = lib.b200_ctc_crf_sparse_fwd(_ptr(scores), t, n, int(state_len), _semiring(semiring, what), _ptr(logz),
+                                         _ptr(alpha), _ptr(workspace), _stream(stream))
+    _check(rc, "b200_ctc_crf_sparse_fwd")
+    return logz
+
+
+def ctc_crf_sparse_bwd(scores, state_len, semiring, beta, stream=None):
+    """k-mer lattice backward scores beta [T+1, N, S] (see b200_ctc_crf_sparse_bwd)."""
+    lib = require()
+    what = "ctc_crf_sparse_bwd"
+    t, n = _sparse_shape(scores, state_len, what)
+    _dev(beta, torch.float32, "beta", what, (t + 1, n, 4 ** state_len))
+    with torch.cuda.device(scores.device):
+        rc = lib.b200_ctc_crf_sparse_bwd(_ptr(scores), t, n, int(state_len), _semiring(semiring, what), _ptr(beta),
+                                         _stream(stream))
+    _check(rc, "b200_ctc_crf_sparse_bwd")
+    return beta
+
+
+def ctc_crf_sparse_grad(scores, state_len, semiring, g, workspace, grad, stream=None):
+    """grad [T, N, C] = g[n] * dlogz[n]/dscores from the workspace of ctc_crf_sparse_fwd (see b200_ctc_crf_sparse_grad)."""
+    lib = require()
+    what = "ctc_crf_sparse_grad"
+    t, n = _sparse_shape(scores, state_len, what)
+    _dev(g, torch.float32, "g", what, (n,))
+    _dev(grad, torch.float32, "grad", what, tuple(scores.shape))
+    _dev(workspace, torch.uint8, "workspace", what)
+    need = ctc_crf_sparse_workspace_bytes(n, t, state_len, semiring)
+    if workspace.numel() < need:
+        raise NativeError(f"{what}: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(scores.device):
+        rc = lib.b200_ctc_crf_sparse_grad(_ptr(scores), t, n, int(state_len), _semiring(semiring, what), _ptr(g),
+                                          _ptr(workspace), _ptr(grad), _stream(stream))
+    _check(rc, "b200_ctc_crf_sparse_grad")
+    return grad
+
+
+def ctc_crf_target_max_states():
+    return load().b200_ctc_crf_target_max_states()
+
+
+def ctc_crf_target_workspace_bytes(n, t, l, semiring):
+    return load().b200_ctc_crf_target_workspace_bytes(int(n), int(t), int(l), int(semiring))
+
+
+def _target_shape(stay, move, lengths, what):
+    _dev(stay, torch.float32, "stay", what)
+    if stay.dim() != 3:
+        raise NativeError(f"{what}: stay must be [T, N, L], got {tuple(stay.shape)}")
+    t, n, l = stay.shape
+    _dev(move, torch.float32, "move", what, (t, n, l - 1))
+    _dev(lengths, torch.int32, "lengths", what, (n,))
+    return t, n, l
+
+
+def ctc_crf_target_fwd(stay, move, lengths, semiring, logz, workspace=None, stream=None):
+    """Target-lattice logZ (see b200_ctc_crf_target_fwd): stay [T, N, L], move [T, N, L-1] fp32, lengths [N] int32 ->
+    logz [N]; `workspace` (ctc_crf_target_workspace_bytes bytes) keeps what ctc_crf_target_grad needs."""
+    lib = require()
+    what = "ctc_crf_target_fwd"
+    t, n, l = _target_shape(stay, move, lengths, what)
+    _dev(logz, torch.float32, "logz", what, (n,))
+    if workspace is not None:
+        _dev(workspace, torch.uint8, "workspace", what)
+        need = ctc_crf_target_workspace_bytes(n, t, l, semiring)
+        if workspace.numel() < need:
+            raise NativeError(f"{what}: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(stay.device):
+        rc = lib.b200_ctc_crf_target_fwd(_ptr(stay), _ptr(move), _ptr(lengths), t, n, l, _semiring(semiring, what),
+                                         _ptr(logz), _ptr(workspace), _stream(stream))
+    _check(rc, "b200_ctc_crf_target_fwd")
+    return logz
+
+
+def ctc_crf_target_grad(stay, move, lengths, semiring, g, workspace, dstay, dmove, stream=None):
+    """dstay / dmove = g[n] * dlogz[n]/d(stay, move) from the workspace of ctc_crf_target_fwd (see b200_ctc_crf_target_grad)."""
+    lib = require()
+    what = "ctc_crf_target_grad"
+    t, n, l = _target_shape(stay, move, lengths, what)
+    _dev(g, torch.float32, "g", what, (n,))
+    _dev(dstay, torch.float32, "dstay", what, (t, n, l))
+    _dev(dmove, torch.float32, "dmove", what, (t, n, l - 1))
+    _dev(workspace, torch.uint8, "workspace", what)
+    need = ctc_crf_target_workspace_bytes(n, t, l, semiring)
+    if workspace.numel() < need:
+        raise NativeError(f"{what}: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(stay.device):
+        rc = lib.b200_ctc_crf_target_grad(_ptr(stay), _ptr(move), _ptr(lengths), t, n, l, _semiring(semiring, what),
+                                          _ptr(g), _ptr(workspace), _ptr(dstay), _ptr(dmove), _stream(stream))
+    _check(rc, "b200_ctc_crf_target_grad")
+    return dstay, dmove
 
 
 def lstm_crf_fwd(plan_struct, x, scores, stream=None):

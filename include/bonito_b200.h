@@ -18,6 +18,8 @@
  *   b200_crf_decode           koi.decode.beam_search call contract    bonito/crf/basecall.py:36-40
  *                             with SeqdistModel.decode_batch maths    bonito/crf/model.py:98-108,196-199
  *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
+ *   b200_ctc_crf_*            koi.ctc (logZ_cu_sparse, fwd/bwd_scores_  bonito/crf/model.py:30-143
+ *                             cu_sparse, logZ_cu, viterbi_alignments)
  *
  * Conventions (SURVEY.md section 8b): every function returns 0 on success and a negative value on
  * failure, with a message available from b200_last_error().  All pointers are raw DEVICE pointers
@@ -361,6 +363,44 @@ int b200_lstm_crf_fwd(const b200_lstm_crf_plan* plan, const void* x, void* score
  */
 int b200_crf_beam_search(const void* scores, int n, int t, int state_len, float blank_score, int beam_width, float beam_cut,
                          float qscale, float qbias, void* workspace, void* moves, void* sequence, void* qstring, void* stream);
+
+/*
+ * ---- CTC-CRF sequence distribution (reference: CTC_CRF, bonito/crf/model.py:30-143, on koi.ctc's logZ_cu_sparse,
+ *      fwd/bwd_scores_cu_sparse, logZ_cu and viterbi_alignments) ----
+ * All tensors fp32 (lengths int32), contiguous, on the device; `semiring` is B200_SEMIRING_LOG (logsumexp) or
+ * B200_SEMIRING_MAX.  Every output is written in full and is bitwise reproducible.
+ *
+ * The k-mer lattice: S = 4^state_len states (state_len 1..5), scores [t][n][5*S] 16-byte aligned, the edge from
+ * idx[s][e] into s at column s*5 + e (idx[s][0] = s, idx[s][1+j] = j*S/4 + s/4); alpha_0 = beta_t = 0 for every state.
+ *   b200_ctc_crf_sparse_fwd:  logz [n]; alpha [t+1][n][S] when not NULL; when `workspace` is not NULL (of
+ *     b200_ctc_crf_sparse_workspace_bytes(n, t, state_len, semiring) bytes) it keeps what b200_ctc_crf_sparse_grad needs.
+ *   b200_ctc_crf_sparse_bwd:  beta [t+1][n][S].
+ *   b200_ctc_crf_sparse_grad: grad [t][n][5*S] = g[c] * dlogz[c]/dscores from the workspace of a forward with the same
+ *     arguments.  Log: g * exp(alpha_t[idx[s][e]] + scores[t][c][s*5+e] + beta_{t+1}[s] - logz); Max: g on the edges of
+ *     the best path (ties: the lowest in-edge at every frame, then the lowest final state), 0 elsewhere.
+ *
+ * The target lattice of ctc_loss: stay [t][n][l], move [t][n][l-1], lengths [n] (target_lengths + 1 - state_len), l <=
+ * b200_ctc_crf_target_max_states();  alpha_0 = [0, -inf, ...], alpha_{u+1}[j] = alpha_u[j] * stay[u][j] (+)
+ * alpha_u[j-1] * move[u][j-1] (semiring product and sum), logz = alpha_t[lengths-1].  A chunk with lengths < 1,
+ * lengths > l or lengths - 1 > t is infeasible: logz = -inf and a gradient of exactly 0.
+ *   b200_ctc_crf_target_fwd:  logz [n]; `workspace` (b200_ctc_crf_target_workspace_bytes bytes) as above, or NULL.
+ *   b200_ctc_crf_target_grad: dstay [t][n][l], dmove [t][n][l-1] = g[c] * dlogz[c]/d(stay, move); Max: g on the edges
+ *     of the best path, ties to the stay.
+ */
+#define B200_SEMIRING_LOG 0
+#define B200_SEMIRING_MAX 1
+size_t b200_ctc_crf_sparse_workspace_bytes(int n, int t, int state_len, int semiring);
+int b200_ctc_crf_sparse_fwd(const void* scores, int t, int n, int state_len, int semiring, void* logz, void* alpha,
+                            void* workspace, void* stream);
+int b200_ctc_crf_sparse_bwd(const void* scores, int t, int n, int state_len, int semiring, void* beta, void* stream);
+int b200_ctc_crf_sparse_grad(const void* scores, int t, int n, int state_len, int semiring, const void* g,
+                             void* workspace, void* grad, void* stream);
+int b200_ctc_crf_target_max_states(void);
+size_t b200_ctc_crf_target_workspace_bytes(int n, int t, int l, int semiring);
+int b200_ctc_crf_target_fwd(const void* stay, const void* move, const void* lengths, int t, int n, int l, int semiring,
+                            void* logz, void* workspace, void* stream);
+int b200_ctc_crf_target_grad(const void* stay, const void* move, const void* lengths, int t, int n, int l, int semiring,
+                             const void* g, void* workspace, void* dstay, void* dmove, void* stream);
 
 #ifdef __cplusplus
 }
