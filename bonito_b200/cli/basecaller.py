@@ -4,8 +4,11 @@
 Alignment (`--reference`, needs mappy) and CTC training-data export (`--save-ctc`) are outside the hot path and
 exit with an explanation; output is unaligned FASTQ, or unaligned SAM text with the `mv:B:c` move table when stdout is
 redirected to a `.sam` file (the reference's `biofmt` rule, bonito/io.py:35-54).
+`B200_CTC_BEAMSIZE=W` in the environment (1..32, unset = 1, the greedy decode) decodes the QuartzNet CTC models with the
+prefix beam search of width W; the flag surface itself is the reference's and has no beam option.
 """
 
+import os
 import sys
 from argparse import ArgumentParser, ArgumentDefaultsHelpFormatter
 from datetime import timedelta
@@ -14,7 +17,7 @@ from time import perf_counter
 
 import numpy as np
 
-from bonito_b200.ctc.model import Model as CtcModel
+from bonito_b200.ctc.model import MAX_BEAMSIZE, Model as CtcModel
 from bonito_b200.io import Writer, biofmt
 from bonito_b200.nn import fuse_bn_
 from bonito_b200.reader import Reader
@@ -59,6 +62,13 @@ def main(args):
     if args.revcomp and isinstance(model, CtcModel):
         sys.stderr.write("> error: --revcomp is not supported for the QuartzNet CTC models (dna_r9.4.1@v1, @v2)\n")
         exit(1)
+    decode_args = {}
+    if isinstance(model, CtcModel):
+        width = os.environ.get("B200_CTC_BEAMSIZE", "1")
+        if not width.isdigit() or not 1 <= int(width) <= MAX_BEAMSIZE:
+            sys.stderr.write(f"> error: B200_CTC_BEAMSIZE must be an integer in 1..{MAX_BEAMSIZE}, got '{width}'\n")
+            exit(1)
+        decode_args["beamsize"] = int(width)
     try:
         # build the native plan now: a layer stack without a native kernel is reported here, not from the writer thread
         model.native_plan()
@@ -80,8 +90,7 @@ def main(args):
 
     params = model.config["basecaller"]
     results = basecall(model, reads, reverse=args.revcomp, rna=args.rna, batchsize=params["batchsize"],
-                       chunksize=params["chunksize"], overlap=params["overlap"])
-    import os
+                       chunksize=params["chunksize"], overlap=params["overlap"], **decode_args)
     writer = Writer(results, min_qscore=args.min_qscore, mode=fmt.mode,
                     group_key=os.path.basename(os.path.normpath(args.model_directory)))
     t0 = perf_counter()

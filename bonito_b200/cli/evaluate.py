@@ -5,8 +5,9 @@ flag surface and the printed summary of the reference's `bonito evaluate` (bonit
 Each batch of chunks runs the native forward and decode; the calls are aligned to their references by one batched
 Smith-Waterman launch on the GPU (`bonito_b200.align`; the scoring and tie rules are in bonito_b200/csrc/align.cu).
 Deviations from the reference:
-  * CTC models (QuartzNet) are decoded greedily; the reference decodes them with a width-5 beam search, so their
-    accuracies here are greedy accuracies.
+  * CTC models (QuartzNet) are decoded greedily, so their accuracies here are greedy accuracies; the reference decodes
+    them with a width-5 beam search.  The package has a CTC beam search (`bonito_b200.ctc.model.beam_search`, `basecall(...,
+    beamsize=W)`), but `evaluate` does not use it: its flags and outputs are the reference's and have no decode switch.
   * a chunk whose call shares no base with its reference reports accuracy 0 (the reference raises ZeroDivisionError).
   * alignment ties follow this project's rules, not parasail's (which nothing pins); among co-optimal alignments the
     counts almost never differ.

@@ -73,6 +73,11 @@ int launch_ctc_crf_target_fwd(const float* stay, const float* move, const int* l
 int launch_ctc_crf_target_grad(const float* stay, const float* move, const int* lengths, int T, int N, int L, int semiring,
                                const float* g, void* workspace, float* dstay, float* dmove, cudaStream_t stream);
 
+size_t ctc_beam_workspace_bytes(int n_reads, long long total_frames, int beam_width);
+int launch_ctc_beam_search(const __half* logp, const long long* frame_off, const int* frame_len, int n_reads, int beam_width,
+                           float threshold, float qscale, float qbias, void* workspace, size_t workspace_bytes,
+                           uint8_t* sequence, uint8_t* qstring, uint8_t* moves, cudaStream_t stream);
+
 int launch_quantize_i8(const __half* x, int8_t* out, long long n, float scale, cudaStream_t stream);
 int launch_gemm_i8(const int8_t* A, long long lda, const int8_t* B, const float* col_scale, __half* C, long long ldc, int M,
                    int N, int K, const GemmEpilogue& ep, int max_ctas, cudaStream_t stream);
@@ -431,6 +436,18 @@ int b200_ctc_crf_target_grad(const void* stay, const void* move, const void* len
     if (n == 0) return 0;
     return launch_ctc_crf_target_grad((const float*)stay, (const float*)move, (const int*)lengths, t, n, l, semiring,
                                       (const float*)g, workspace, (float*)dstay, (float*)dmove, (cudaStream_t)stream);
+}
+
+size_t b200_ctc_beam_workspace_bytes(int n_reads, long long total_frames, int beam_width) {
+    return ctc_beam_workspace_bytes(n_reads, total_frames, beam_width);
+}
+
+int b200_ctc_beam_search(const void* logp, const long long* frame_off, const int* frame_len, int n_reads, int beam_width,
+                         float threshold, float qscale, float qbias, void* workspace, size_t workspace_bytes, void* sequence,
+                         void* qstring, void* moves, void* stream) {
+    return launch_ctc_beam_search((const __half*)logp, frame_off, frame_len, n_reads, beam_width, threshold, qscale, qbias,
+                                  workspace, workspace_bytes, (uint8_t*)sequence, (uint8_t*)qstring, (uint8_t*)moves,
+                                  (cudaStream_t)stream);
 }
 
 }  // extern "C"

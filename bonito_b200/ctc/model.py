@@ -6,6 +6,12 @@ the same attribute names and registration order), so a reference `weights_N.tar`
 BatchNorm running statistics included.  On the CPU without `use_koi` the module tree runs and returns `[T, N, 5]`
 log-probs, as the reference's `forward` does.  With `use_koi` the native engine (`bonito_b200.engine_ctc.CtcPlan`) runs
 it on the GPU and returns batch-first `[N, T, 5]` fp16 log-probs; there is no eager CUDA path.
+
+Decoding: `greedy_step` / `greedy_collapse` (host, the default) and `beam_search`, the CTC prefix beam search on the GPU
+(`b200_ctc_beam_search`; cut, merge, tie, move and quality rules in bonito_b200/csrc/ctc_beam.cu).  The reference decodes
+with fast_ctc_decode's beam search of width 5 (bonito/ctc/model.py:39-46).  Deviations: the default here is the greedy
+decode; the beam search returns qualities and emission frames, which the reference's has not, so `qscores=True` keeps the
+beam search where the reference switches to its Viterbi decode; there is no CPU path for the beam search.
 """
 
 import numpy as np
@@ -75,23 +81,67 @@ class Model(Module):
         self._native = dict(kwargs)
         self._plan = None
 
-    def decode(self, x, beamsize=1, qscores=False, return_path=False):
+    def decode(self, x, beamsize=1, threshold=1e-3, qscores=False, return_path=False):
         """
-        Greedy CTC decode of one `[T, 5]` log-prob tensor (see `greedy_collapse`).  Returns the sequence, with the quality
-        string appended when `qscores` (the layout of the reference's viterbi_search), and the emission frames when
-        `return_path`.  The CTC prefix beam search (`beamsize > 1`) is not implemented.
+        Decode one `[T, 5]` log-prob tensor: greedily on the host with `beamsize=1` (see `greedy_collapse`), with the prefix
+        beam search on the GPU with `beamsize` in 2..32 (`beam_search`; x must be a CUDA tensor, `threshold` is its
+        probability cut).  Returns the sequence, with the quality string appended when `qscores` (the layout of the
+        reference's viterbi_search), and the emission frames when `return_path`.  `qscores` does not change the sequence:
+        the beam search has qualities of its own (the reference's has none and falls back to Viterbi).
         """
-        if beamsize != 1:
-            raise NotImplementedError("CTC beam search is not implemented; use beamsize=1")
-        logp = x.detach().float().cpu().numpy()
-        labels, probs = greedy_step(logp)
-        seq, qstring, moves = greedy_collapse(labels, probs, self.alphabet, self.qscale, self.qbias)
+        check_beamsize(beamsize)
+        if beamsize > 1:
+            check_alphabet(self.alphabet)
+            seq, qstring, moves = beam_search(x.detach(), [0, x.shape[0]], beamsize, threshold, self.qscale, self.qbias).cpu().numpy()
+        else:
+            logp = x.detach().float().cpu().numpy()
+            labels, probs = greedy_step(logp)
+            seq, qstring, moves = greedy_collapse(labels, probs, self.alphabet, self.qscale, self.qbias)
         seq = seq[seq != 0].tobytes().decode()
         if qscores:
             seq += qstring[qstring != 0].tobytes().decode()
         if return_path:
             return seq, np.flatnonzero(moves)
         return seq
+
+
+MAX_BEAMSIZE = 32
+
+
+def check_beamsize(beamsize):
+    if not isinstance(beamsize, int) or not 1 <= beamsize <= MAX_BEAMSIZE:
+        raise ValueError(f"beamsize must be an integer in 1..{MAX_BEAMSIZE}, got {beamsize!r}")
+
+
+def check_alphabet(alphabet):
+    if "".join(alphabet) != "NACGT":
+        raise ValueError(f"the CTC beam search writes the bases of the alphabet NACGT, the model has {''.join(alphabet)!r}")
+
+
+def beam_search(logp, offsets, beamsize=5, threshold=1e-3, qscale=1.0, qbias=0.0):
+    """
+    CTC prefix beam search of a batch of reads in one launch of `b200_ctc_beam_search`.  `logp`: CUDA `[frames, 5]`
+    log-probs (class 0 = blank) of the reads packed back to back; `offsets`: the len(reads) + 1 frame boundaries, read r
+    being frames offsets[r]:offsets[r + 1].  Returns a CUDA uint8 tensor `[3, frames]` = sequence, qstring, moves in the
+    byte layout of `greedy_collapse`.  There is no CPU path.
+    """
+    from bonito_b200 import native
+    check_beamsize(beamsize)
+    if not isinstance(logp, torch.Tensor) or not logp.is_cuda:
+        raise NotImplementedError("CTC beam search has no CPU path: it needs CUDA log-probs (use beamsize=1 for the greedy decode)")
+    if logp.dim() != 2 or logp.shape[1] != 5:
+        raise ValueError(f"beam_search: logp must be [frames, 5], got {tuple(logp.shape)}")
+    offsets = np.asarray(offsets, dtype=np.int64)
+    if offsets.ndim != 1 or offsets.size < 1 or offsets[0] != 0 or offsets[-1] != logp.shape[0] or (np.diff(offsets) < 0).any():
+        raise ValueError("beam_search: offsets must rise from 0 to the number of frames")
+    logp = logp.to(torch.float16).contiguous()
+    frames, reads = logp.shape[0], offsets.size - 1
+    with torch.cuda.device(logp.device):
+        out = torch.empty(3, frames, dtype=torch.uint8, device=logp.device)
+        workspace = torch.empty(native.ctc_beam_workspace_bytes(reads, frames, beamsize), dtype=torch.uint8, device=logp.device)
+        native.ctc_beam_search(logp, offsets[:-1], np.diff(offsets), beamsize, threshold, qscale, qbias, workspace,
+                               out[0], out[1], out[2])
+    return out
 
 
 def greedy_step(logp):

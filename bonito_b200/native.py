@@ -104,6 +104,9 @@ SIGNATURES = {
                                         c_void_p]),
     "b200_ctc_crf_target_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_beam_workspace_bytes": (c_size_t, [c_int, c_longlong, c_int]),
+    "b200_ctc_beam_search": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_float, c_void_p, c_size_t,
+                                     c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 
@@ -615,6 +618,42 @@ def ctc_crf_target_grad(stay, move, lengths, semiring, g, workspace, dstay, dmov
                                           _ptr(g), _ptr(workspace), _ptr(dstay), _ptr(dmove), _stream(stream))
     _check(rc, "b200_ctc_crf_target_grad")
     return dstay, dmove
+
+
+def ctc_beam_workspace_bytes(n_reads, total_frames, beam_width):
+    return load().b200_ctc_beam_workspace_bytes(int(n_reads), int(total_frames), int(beam_width))
+
+
+def ctc_beam_search(logp, frame_off, frame_len, beam_width, threshold, qscale, qbias, workspace, sequence, qstring, moves,
+                    stream=None):
+    """CTC prefix beam search over packed reads (see b200_ctc_beam_search): logp CUDA fp16 [frames, 5]; frame_off int64 and
+    frame_len int32 host arrays of one entry per read (copied into the workspace on `stream` before this returns);
+    workspace CUDA uint8 of ctc_beam_workspace_bytes(n_reads, sum(frame_len), beam_width) bytes; sequence / qstring /
+    moves CUDA uint8 [frames]."""
+    lib = require()
+    what = "ctc_beam_search"
+    _dev(logp, torch.float16, "logp", what)
+    if logp.dim() != 2 or logp.shape[1] != 5:
+        raise NativeError(f"{what}: logp must be [frames, 5], got {tuple(logp.shape)}")
+    frames = logp.shape[0]
+    ln = np.ascontiguousarray(frame_len, dtype=np.int32)
+    off = np.ascontiguousarray(frame_off, dtype=np.int64)
+    if ln.ndim != 1 or off.shape != ln.shape:
+        raise NativeError(f"{what}: frame_off and frame_len must have one entry per read, got shapes {off.shape} / {ln.shape}")
+    n = ln.shape[0]
+    if n and (int(ln.min()) < 0 or int(off.min()) < 0 or int((off + ln).max()) > frames):
+        raise NativeError(f"{what}: a read lies outside the {frames} frames of logp")
+    if not 1 <= int(beam_width) <= 32:
+        raise NativeError(f"{what}: beam_width {beam_width} is outside [1, 32]")
+    for t, name in ((sequence, "sequence"), (qstring, "qstring"), (moves, "moves")):
+        _dev(t, torch.uint8, name, what, (frames,))
+    _dev(workspace, torch.uint8, "workspace", what)
+    with torch.cuda.device(logp.device):
+        rc = lib.b200_ctc_beam_search(_ptr(logp), off.ctypes.data, ln.ctypes.data, n, int(beam_width), float(threshold),
+                                      float(qscale), float(qbias), _ptr(workspace), workspace.numel(), _ptr(sequence),
+                                      _ptr(qstring), _ptr(moves), _stream(stream))
+    _check(rc, "b200_ctc_beam_search")
+    return sequence, qstring, moves
 
 
 def lstm_crf_fwd(plan_struct, x, scores, stream=None):

@@ -20,6 +20,7 @@
  *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
  *   b200_ctc_crf_*            koi.ctc (logZ_cu_sparse, fwd/bwd_scores_  bonito/crf/model.py:30-143
  *                             cu_sparse, logZ_cu, viterbi_alignments)
+ *   b200_ctc_beam_search      fast_ctc_decode.beam_search             bonito/ctc/model.py:39-46, ctc/basecall.py:43-61
  *
  * Conventions (SURVEY.md section 8b): every function returns 0 on success and a negative value on
  * failure, with a message available from b200_last_error().  All pointers are raw DEVICE pointers
@@ -401,6 +402,27 @@ int b200_ctc_crf_target_fwd(const void* stay, const void* move, const void* leng
                             void* logz, void* workspace, void* stream);
 int b200_ctc_crf_target_grad(const void* stay, const void* move, const void* lengths, int t, int n, int l, int semiring,
                              const void* g, void* workspace, void* dstay, void* dmove, void* stream);
+
+/*
+ * ---- CTC prefix beam search (reference: fast_ctc_decode.beam_search behind bonito/ctc/model.py:39-46; that crate's output
+ *      is pinned by nothing here, so the cut, merge, tie, move and quality rules are this library's, stated in
+ *      bonito_b200/csrc/ctc_beam.cu) ----
+ * logp: DEVICE fp16 [frames][5] log-probs (class 0 = blank, 1..4 = A C G T) of n_reads reads packed along the frame axis;
+ * read r is frames [frame_off[r], frame_off[r] + frame_len[r]).  As for b200_sw_align, frame_off (int64) and frame_len
+ * (int32) are HOST arrays, checked on the host (0 <= frame_len <= 2^26, else -2) and copied into the head of `workspace`
+ * on `stream`.  beam_width in [1, 32]; a class whose probability is below `threshold` (in [0, 1], the reference uses 1e-3)
+ * is skipped at that frame.
+ * workspace: DEVICE memory of workspace_bytes >= b200_ctc_beam_workspace_bytes(n_reads, sum of frame_len, beam_width)
+ * bytes (the per-read arrays plus 1 + beam_width * frame_len[r] prefix nodes of 8 bytes per read); a smaller one returns
+ * -2 with the sizes in the message before anything is launched.
+ * sequence / qstring / moves: DEVICE bytes indexed like the frames of logp; every frame of every read is written: the base
+ * ('A' 'C' 'G' 'T'), its quality character and 1 on the frame where a base of the answer entered the beam, 0 elsewhere
+ * (the byte layout of b200_crf_decode).  Frames outside the reads are not touched.  Bitwise reproducible.
+ */
+size_t b200_ctc_beam_workspace_bytes(int n_reads, long long total_frames, int beam_width);
+int b200_ctc_beam_search(const void* logp, const long long* frame_off, const int* frame_len, int n_reads, int beam_width,
+                         float threshold, float qscale, float qbias, void* workspace, size_t workspace_bytes, void* sequence,
+                         void* qstring, void* moves, void* stream);
 
 #ifdef __cplusplus
 }
