@@ -95,6 +95,14 @@ __device__ __forceinline__ void bulk_copy_to_peer(uint32_t peer_dst, uint32_t lo
                      "r"(peer_dst), "r"(local_src), "r"(bytes), "r"(peer_bar)
                  : "memory");
 }
+// 2-D tensor copy global -> own shared memory (TMA engine) at element coordinates (c0 innermost, c1); elements outside
+// the tensor are zero-filled and still count towards the `bytes` completed on the mbarrier
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint32_t bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
+        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(bar)
+        : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 // make generic-proxy writes (st.shared / st.shared::cluster) visible to the async proxy (wgmma / bulk-copy reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;\n" ::: "memory"); }
@@ -108,6 +116,17 @@ __device__ __forceinline__ uint64_t wg_desc_noswz(uint32_t smem_addr, uint32_t l
     d |= (uint64_t)(lbo >> 4) << 16;               // leading byte offset  bits [16,30)
     d |= (uint64_t)(sbo >> 4) << 32;               // stride byte offset   bits [32,46)
     return d;                                      // layout type 0 (no swizzle) in bits [62,64)
+}
+// K-major tile with the 128-byte swizzle (what a TMA copy with CU_TENSOR_MAP_SWIZZLE_128B writes): rows of 128 bytes,
+// 8-row atoms 1024 bytes apart (sbo), the atom 1024-byte aligned.  A k-step inside the row adds its byte offset to the
+// start address.
+__device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address                     bits [0,14)
+    d |= (uint64_t)1 << 16;                        // leading byte offset (unused: K-major swizzled)
+    d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset                bits [32,46)
+    d |= (uint64_t)1 << 62;                        // layout type 1: 128-byte swizzle   bits [62,64)
+    return d;
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }

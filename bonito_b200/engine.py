@@ -757,7 +757,8 @@ class LstmCrfPlan:
         if self.tile and os.environ.get("B200_LSTM_TILE", "1") != "0":
             if tiled is None:
                 # Default: the layer-by-layer schedule (14 launches per batch).  With two batches in flight on two streams
-                # (score_batches, bench.py) it measured faster than per-tile streams (17.8 vs 18.8 ms per 512-chunk batch):
+                # (score_batches, bench.py) it measured faster than per-tile streams on an H100 80GB HBM3 at 700 W (bench.py
+                # hac step, two 512-chunk batches in flight: 62.2 / 62.7 ms, one repeat at 73.7 ms, vs 66.1 / 66.1 ms):
                 # the GEMMs / decode of one batch fill the SMs the other batch's recurrent clusters leave free.
                 tiled = (not return_features) and x.shape[0] > self.tile and os.environ.get("B200_TILE_STREAMS", "0") != "0"
             return self.forward_tiles(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features,
