@@ -1,9 +1,10 @@
 """
 `bonito_b200 basecaller <model_directory> <reads_directory>` -- the flag surface of the reference's
 `bonito basecaller` (`bonito/cli/basecaller.py:168-199`) over the native engine.
-Alignment (`--reference`, needs mappy) and CTC training-data export (`--save-ctc`) are outside the hot path and
-exit with an explanation; output is unaligned FASTQ, or unaligned SAM text with the `mv:B:c` move table when stdout is
-redirected to a `.sam` file (the reference's `biofmt` rule, bonito/io.py:35-54).
+Output is FASTQ, or SAM text with the `mv:B:c` move table when stdout is redirected to a `.sam` file (the reference's
+`biofmt` rule, bonito/io.py:35-54).  `--reference <fasta>` maps the calls on the GPU (bonito_b200.aligner, this
+project's rules in place of minimap2's) and writes aligned SAM; `--alignment-threads` is accepted and has no effect.  CTC
+training-data export (`--save-ctc`) exits with an explanation.
 `B200_CTC_BEAMSIZE=W` in the environment (1..32, unset = 1, the greedy decode) decodes the QuartzNet CTC models with the
 prefix beam search of width W; the flag surface itself is the reference's and has no beam option.
 """
@@ -17,6 +18,7 @@ from time import perf_counter
 
 import numpy as np
 
+from bonito_b200.aligner import PRESETS, Aligner, IndexBuildError, align_map
 from bonito_b200.ctc.model import MAX_BEAMSIZE, Model as CtcModel
 from bonito_b200.io import Writer, biofmt
 from bonito_b200.nn import fuse_bn_
@@ -33,8 +35,11 @@ def _column_to_set(filename, idx=0):
 
 def main(args):
     init(args.seed, args.device)
-    if args.reference or args.save_ctc:
-        sys.stderr.write("> error: --reference / --save-ctc need minimap2 (mappy), which this build does not bundle\n")
+    if args.save_ctc:
+        sys.stderr.write("> error: --save-ctc (CTC training data) is not supported by this build\n")
+        exit(1)
+    if args.reference and args.mm2_preset not in PRESETS:
+        sys.stderr.write(f"> error: unknown --mm2-preset '{args.mm2_preset}', choose one of {', '.join(PRESETS)}\n")
         exit(1)
     try:
         reader = Reader(args.reads_directory, args.recursive)
@@ -42,11 +47,14 @@ def main(args):
     except FileNotFoundError:
         sys.stderr.write("> error: no suitable files found in %s\n" % args.reads_directory)
         exit(1)
-    fmt = biofmt(aligned=False)
+    fmt = biofmt(aligned=args.reference is not None)
     if fmt.mode not in ("wfq", "w"):
         sys.stderr.write(f"> error: {fmt.name} output needs htslib, which this build does not bundle; redirect to .sam or .fastq\n")
         exit(1)
-    sys.stderr.write(f"> outputting {fmt.aligned} {fmt.name}\n")
+    if args.reference and fmt.name == "fastq":
+        sys.stderr.write(f"> warning: did you really want {fmt.aligned} {fmt.name}?\n")
+    else:
+        sys.stderr.write(f"> outputting {fmt.aligned} {fmt.name}\n")
     sys.stderr.write(f"> loading model {args.model_directory}\n")
     try:
         model = load_model(args.model_directory, args.device, weights=args.weights if args.weights > 0 else None,
@@ -79,6 +87,14 @@ def main(args):
         sys.stderr.write(f"> model basecaller params: {model.config['basecaller']}\n")
 
     basecall = load_symbol(args.model_directory, "basecall")
+    aligner = None
+    if args.reference and fmt.name != "fastq":       # FASTQ has no alignment fields: the mapping is skipped
+        sys.stderr.write("> loading reference\n")
+        try:
+            aligner = Aligner(args.reference, preset=args.mm2_preset, device=args.device)
+        except IndexBuildError:
+            sys.stderr.write("> failed to load/build index\n")
+            exit(1)
     scaling = model.config.get("scaling")
     pa = bool(scaling) and scaling.get("strategy") == "pa"
     reads = reader.get_reads(
@@ -91,8 +107,11 @@ def main(args):
     params = model.config["basecaller"]
     results = basecall(model, reads, reverse=args.revcomp, rna=args.rna, batchsize=params["batchsize"],
                        chunksize=params["chunksize"], overlap=params["overlap"], **decode_args)
+    if aligner:
+        results = align_map(aligner, results, n_thread=args.alignment_threads)
     writer = Writer(results, min_qscore=args.min_qscore, mode=fmt.mode,
-                    group_key=os.path.basename(os.path.normpath(args.model_directory)))
+                    group_key=os.path.basename(os.path.normpath(args.model_directory)),
+                    contigs=aligner.contigs if aligner else None)
     t0 = perf_counter()
     writer.start()
     writer.join()

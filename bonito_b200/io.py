@@ -1,9 +1,11 @@
 """
-pysam-free output for `bonito_b200 basecaller`: unaligned FASTQ and unaligned SAM text with the reference's header, record
-and tag layout (`bonito/io.py:41-166,400-469`, `documentation/SAM.md`), including the
+pysam-free output for `bonito_b200 basecaller`: FASTQ and SAM text (unaligned, or aligned by bonito_b200.aligner) with the
+reference's header, record and tag layout (`bonito/io.py:41-166,400-469`, `documentation/SAM.md`), including the
 sequence-to-signal move table `mv:B:c,<stride>,<moves...>` (`io.py:57-70,455-456`).  The reference writes through
-pysam / htslib (and aligns with mappy); BAM / CRAM need htslib and alignment needs minimap2, neither of which this build
-bundles, so those formats are refused with an explanation instead of being approximated.
+pysam / htslib; BAM / CRAM need htslib, which this build does not bundle, so those formats are refused with an
+explanation instead of being approximated.
+Deviation: on the reverse strand QUAL is reversed along with SEQ, as the SAM specification requires; the reference
+reverse-complements SEQ and leaves QUAL as called.
 """
 
 import os
@@ -14,6 +16,7 @@ from threading import Thread
 
 import numpy as np
 
+from bonito_b200.aligner import revcomp
 from bonito_b200.util import mean_qscore_from_qstring
 
 __ont_bam_spec__ = "0.0.2"
@@ -66,19 +69,32 @@ def write_fastq(header, sequence, qstring, fd=sys.stdout, tags=None, sep="\t"):
     fd.write(f"{sequence}\n+\n{qstring}\n")
 
 
-def sam_header(groups=(), sep="\t", argv=None):
-    """@HD + @PG basecaller (+ read groups); no aligner @PG line: this build does not align (reference: io.py:109-133)."""
+def sam_header(groups=(), sep="\t", argv=None, contigs=None):
+    """@HD (+ @SQ per contig) + @PG basecaller (+ @PG aligner when `contigs`, [(name, length)], is given) + read groups
+    (reference: io.py:109-133)."""
     argv = sys.argv[1:] if argv is None else argv
-    hd = sep.join(["@HD", "VN:1.5", "SO:unknown", "ob:%s" % __ont_bam_spec__])
-    pg = sep.join(["@PG", "ID:basecaller", "PN:bonito_b200", "VN:%s" % __version__, "CL:bonito_b200 %s" % " ".join(argv)])
-    return "%s\n" % "\n".join([hd, pg, *groups])
+    lines = [sep.join(["@HD", "VN:1.5", "SO:unknown", "ob:%s" % __ont_bam_spec__])]
+    lines += [sep.join(["@SQ", f"SN:{name}", f"LN:{length}"]) for name, length in contigs or ()]
+    lines.append(sep.join(["@PG", "ID:basecaller", "PN:bonito_b200", "VN:%s" % __version__,
+                           "CL:bonito_b200 %s" % " ".join(argv)]))
+    if contigs:
+        lines.append(sep.join(["@PG", "ID:aligner", "PN:bonito_b200", "VN:%s" % __version__,
+                               "DS:GPU minimizer chaining and banded local alignment"]))
+    return "%s\n" % "\n".join([*lines, *groups])
 
 
 def sam_record(read_id, sequence, qstring, mapping=None, tags=None, sep="\t"):
-    """Unaligned SAM record (flag 4), the layout of the reference's `sam_record` without a mapping (io.py:136-166)."""
+    """SAM record in the layout of the reference's `sam_record` (io.py:136-166): flag 4 without a mapping; with one (a
+    bonito_b200.aligner.Mapping) flag 0 / 16, soft clips in reference orientation, SEQ and QUAL reversed on strand -."""
     if mapping:
-        raise NotImplementedError("aligned output needs minimap2 (mappy), which this build does not bundle")
-    record = [read_id, 4, "*", 0, 0, "*", "*", 0, 0, sequence, qstring, "NM:i:0"]
+        fwd = mapping.strand == +1
+        right = len(sequence) - mapping.q_en
+        clips = ["%dS" % mapping.q_st if mapping.q_st else "", mapping.cigar_str, "%dS" % right if right else ""]
+        record = [read_id, 0 if fwd else 16, mapping.ctg, mapping.r_st + 1, mapping.mapq,
+                  "".join(clips if fwd else clips[::-1]), "*", 0, 0, sequence if fwd else revcomp(sequence),
+                  qstring if fwd else qstring[::-1], "NM:i:%d" % mapping.NM, "MD:Z:%s" % mapping.MD]
+    else:
+        record = [read_id, 4, "*", 0, 0, "*", "*", 0, 0, sequence, qstring, "NM:i:0"]
     if tags is not None:
         record.extend(tags)
     return sep.join(map(str, record))
@@ -140,28 +156,31 @@ class DuplexWriter(Thread):
 class Writer(Thread):
     """
     Drains the basecall iterator on its own thread; `.log` holds (read_id, num_samples) of the reads written.
-    mode "wfq": FASTQ (`tags=True` puts the SAM tags on the header line as the reference does); mode "w": SAM text.
+    mode "wfq": FASTQ (`tags=True` puts the SAM tags on the header line as the reference does); mode "w": SAM text, aligned
+    where a result carries a `mapping` (with `contigs` [(name, length)] for the @SQ header lines).
     """
 
-    def __init__(self, iterator, fd=sys.stdout, min_qscore=0, mode="wfq", groups=(), group_key=None, tags=False):
+    def __init__(self, iterator, fd=sys.stdout, min_qscore=0, mode="wfq", groups=(), group_key=None, tags=False,
+                 contigs=None):
         super().__init__(daemon=True)
         if mode not in ("wfq", "w"):
             raise ValueError(f"output mode {mode!r} needs htslib (BAM / CRAM), which this build does not bundle: "
                              "redirect to a .sam or .fastq file")
         self.iterator, self.fd, self.min_qscore, self.mode = iterator, fd, min_qscore, mode
-        self.groups, self.group_key, self.tags = list(groups), group_key, tags
+        self.groups, self.group_key, self.tags, self.contigs = list(groups), group_key, tags, contigs
         self.log, self.error = [], None
 
     def run(self):
         try:
             if self.mode == "w":
-                self.fd.write(sam_header(self.groups))
+                self.fd.write(sam_header(self.groups, contigs=self.contigs))
             for read, res in self.iterator:
                 seq, qstring = res["sequence"], res["qstring"]
                 samples = len(read.signal) + getattr(read, "trimmed_samples", 0)
                 if len(seq) and mean_qscore_from_qstring(qstring) >= self.min_qscore:
                     if self.mode == "w":
-                        self.fd.write(sam_record(read.read_id, seq, qstring, tags=read_tags(read, res, self.group_key)) + "\n")
+                        self.fd.write(sam_record(read.read_id, seq, qstring, mapping=res.get("mapping"),
+                                                tags=read_tags(read, res, self.group_key)) + "\n")
                     else:
                         write_fastq(read.read_id, seq, qstring, fd=self.fd,
                                     tags=read_tags(read, res, self.group_key, with_moves=False) if self.tags else None)

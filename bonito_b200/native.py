@@ -107,6 +107,15 @@ SIGNATURES = {
     "b200_ctc_beam_workspace_bytes": (c_size_t, [c_int, c_longlong, c_int]),
     "b200_ctc_beam_search": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_float, c_void_p, c_size_t,
                                      c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_map_minimizers": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b200_map_anchors": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p,
+                                 c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_map_chain": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b200_map_extract": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                 c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_map_align_trace_bytes": (c_size_t, [c_int, c_int]),
+    "b200_map_align": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                               c_void_p]),
 }
 
 
@@ -716,3 +725,73 @@ def gemm_i8(a, lda, b, col_scale, bias, c, ldc, m, n, k, act=ACT_NONE, lo=0.0, h
                                   int(cb_width), int(cb_rows), int(max_ctas), _stream(stream))
     _check(rc, "b200_gemm_i8_fwd")
     return c
+
+
+# ------------------------------------------------------------------------------------------------ mapping (map.cu)
+def _map_dev(t, dtype, name, what):
+    if t is None or not t.is_cuda or t.dtype != dtype or not t.is_contiguous():
+        raise NativeError(f"{what}: {name} must be a contiguous CUDA {dtype} tensor")
+    return _ptr(t)
+
+
+def map_minimizers(seq, seq_off, k, w, kmer, mm, stream=None):
+    """mm[p] = hash << 1 | strand of the minimizer at base p, else -1 (see b200_map_minimizers)."""
+    lib = require()
+    n = seq.numel()
+    for t, dtype, name in ((seq, torch.uint8, "seq"), (seq_off, torch.int64, "seq_off"), (kmer, torch.int64, "kmer"),
+                           (mm, torch.int64, "mm")):
+        _map_dev(t, dtype, name, "map_minimizers")
+    if kmer.numel() < n or mm.numel() < n:
+        raise NativeError("map_minimizers: kmer and mm need one entry per base")
+    with torch.cuda.device(seq.device):
+        _check(lib.b200_map_minimizers(_ptr(seq), n, _ptr(seq_off), seq_off.numel() - 1, int(k), int(w), _ptr(kmer), _ptr(mm),
+                                       _stream(stream)), "b200_map_minimizers")
+
+
+def map_anchors(mm, seq_off, k, uniq, start, val, max_occ, count=None, aoff=None, akey=None, aq=None, stream=None):
+    """Anchors per position into `count`, or (count None) the anchors themselves into akey / aq at aoff."""
+    lib = require()
+    with torch.cuda.device(mm.device):
+        _check(lib.b200_map_anchors(_ptr(mm), mm.numel(), _ptr(seq_off), seq_off.numel() - 1, int(k), _ptr(uniq), uniq.numel(),
+                                    _ptr(start), _ptr(val), int(max_occ), _ptr(count), _ptr(aoff), _ptr(akey), _ptr(aq),
+                                    _stream(stream)), "b200_map_anchors")
+
+
+def map_chain(akey, aq, read_aoff, ctg_off, k, f, pred, stream=None):
+    lib = require()
+    for t, dtype, name in ((akey, torch.int64, "akey"), (aq, torch.int32, "aq"), (read_aoff, torch.int64, "read_aoff"),
+                           (ctg_off, torch.int64, "ctg_off"), (f, torch.int32, "f"), (pred, torch.int32, "pred")):
+        _map_dev(t, dtype, name, "map_chain")
+    with torch.cuda.device(akey.device):
+        _check(lib.b200_map_chain(_ptr(akey), _ptr(aq), _ptr(read_aoff), read_aoff.numel() - 1, _ptr(ctg_off),
+                                  ctg_off.numel() - 1, int(k), _ptr(f), _ptr(pred), _stream(stream)), "b200_map_chain")
+
+
+def map_extract(akey, aq, f, pred, order, read_aoff, seq_off, k, max_band, taken, chain, out, stream=None):
+    lib = require()
+    n_reads = read_aoff.numel() - 1
+    if out.shape != (n_reads, 9) or out.dtype != torch.int64:
+        raise NativeError(f"map_extract: out must be int64 ({n_reads}, 9)")
+    with torch.cuda.device(out.device):
+        _check(lib.b200_map_extract(_ptr(akey), _ptr(aq), _ptr(f), _ptr(pred), _ptr(order), _ptr(read_aoff), _ptr(seq_off),
+                                    n_reads, int(k), int(max_band), _ptr(taken), _ptr(chain), _ptr(out), _stream(stream)),
+               "b200_map_extract")
+
+
+def map_align_trace_bytes(query_len, band):
+    return load().b200_map_align_trace_bytes(int(query_len), int(band))
+
+
+def map_align(query, target, chain, meta, max_band, cen, trace, ops, out, stream=None):
+    """Banded local alignment of each pair along its chain (see b200_map_align); meta CUDA int64 [n, 9]."""
+    lib = require()
+    n = meta.shape[0]
+    if meta.shape != (n, 9) or out.shape != (n, 6):
+        raise NativeError("map_align: meta must be (n, 9) and out (n, 6)")
+    for t, dtype, name in ((query, torch.uint8, "query"), (target, torch.uint8, "target"), (chain, torch.int64, "chain"),
+                           (meta, torch.int64, "meta"), (cen, torch.int32, "cen"), (trace, torch.uint8, "trace"),
+                           (ops, torch.uint8, "ops"), (out, torch.int32, "out")):
+        _map_dev(t, dtype, name, "map_align")
+    with torch.cuda.device(out.device):
+        _check(lib.b200_map_align(_ptr(query), _ptr(target), _ptr(chain), _ptr(meta), n, int(max_band), _ptr(cen), _ptr(trace),
+                                  _ptr(ops), _ptr(out), _stream(stream)), "b200_map_align")

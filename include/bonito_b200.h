@@ -424,6 +424,40 @@ int b200_ctc_beam_search(const void* logp, const long long* frame_off, const int
                          float threshold, float qscale, float qbias, void* workspace, size_t workspace_bytes, void* sequence,
                          void* qstring, void* moves, void* stream);
 
+/*
+ * ---- read-to-reference mapping for `basecaller --reference` (the reference maps with minimap2 through mappy; the
+ *      minimizer, anchor, chaining, extraction and alignment rules here are this library's, stated in
+ *      bonito_b200/csrc/map.cu).  Every array is DEVICE memory; int64 unless stated. ----
+ * b200_map_minimizers: seq = n_seqs sequences packed back to back, sequence s at [seq_off[s], seq_off[s + 1]); odd k in
+ *   [3, 31], w in [1, 255].  kmer (scratch) and mm are [n_bases]; mm[p] = hash << 1 | strand of the minimizer at p, else -1.
+ * b200_map_anchors: index = uniq [n_unique] (sorted hashes), start [n_unique + 1], val [start[n_unique]] (position << 1 |
+ *   strand); a hash with more than max_occ entries is skipped.  count != NULL: count (int32 [n_bases]) = anchors per
+ *   position, nothing else written.  count == NULL: aoff [n_bases] (exclusive prefix of count) places each position's
+ *   anchors: akey = read << 33 | strand << 32 | reference position, aq (int32) = query position on that strand.
+ * b200_map_chain: anchors sorted by akey; read r owns [read_aoff[r], read_aoff[r + 1]); contigs are [ctg_off[c],
+ *   ctg_off[c + 1]) of the global reference coordinate.  f, pred: int32 [anchors].
+ * b200_map_extract: order = the anchors sorted by (read, decreasing f, index); taken = uint8 [anchors], zeroed;
+ *   chain = [anchors][2] receives the primary chain's (q, r) of read r at its anchor offset; out = [n_reads][9]: anchors in
+ *   the primary chain, f1, f2, strand, band half-width (<= max_band), q / r of its first and of its last anchor.
+ * b200_map_align: meta = [n_pairs][9]: query offset, m, target offset, n, chain pair offset, chain length, band half-width
+ *   (<= max_band <= 4096), trace byte offset, ops slot offset (m + n bytes).  cen = int32 indexed like query; trace =
+ *   b200_map_align_trace_bytes(m, band) bytes per pair.  out int32 [n_pairs][6] = score, q_st, q_en, t_st, t_en, n_ops; the
+ *   ops ('=', 'X', 'I', 'D', forward order) are the last n_ops bytes of the pair's slot.
+ */
+int b200_map_minimizers(const void* seq, long long n_bases, const long long* seq_off, int n_seqs, int k, int w, void* kmer,
+                        void* mm, void* stream);
+int b200_map_anchors(const void* mm, long long n_bases, const long long* seq_off, int n_seqs, int k, const void* uniq,
+                     long long n_unique, const void* start, const void* val, int max_occ, void* count, const void* aoff,
+                     void* akey, void* aq, void* stream);
+int b200_map_chain(const void* akey, const void* aq, const long long* read_aoff, int n_reads, const long long* ctg_off, int n_ctg,
+                   int k, void* f, void* pred, void* stream);
+int b200_map_extract(const void* akey, const void* aq, const void* f, const void* pred, const void* order,
+                     const long long* read_aoff, const long long* seq_off, int n_reads, int k, int max_band, void* taken,
+                     void* chain, void* out, void* stream);
+size_t b200_map_align_trace_bytes(int query_len, int band);
+int b200_map_align(const void* query, const void* target, const void* chain, const void* meta, int n_pairs, int max_band,
+                   void* cen, void* trace, void* ops, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
