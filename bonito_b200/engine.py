@@ -16,24 +16,34 @@ activation = "tanh" and / or a scale and no Clamp) and packs the weights into th
 column when the head has a fixed blank_score.  A head without one (dna_r9.4.1@v3) learns its blank scores: the scores
 are then `[N, T, 5 * 4^k]` in the CTC_CRF order [state][stay, m0..m3] (b200_crf_decode_lb).  A Clamp behind a (swish)
 convolution (dna_r10.4.1@v4.0) is fused into its epilogue (B200_ACT_SWISH_CLAMP), the Linear in front of the head is one
-more GEMM; these layers and learned blank scores run on the wide path (H = 768, 1024) only.  Anything else raises
+more GEMM; these layers and learned blank scores run on the wide layout (H = 768, 1024) only.  Anything else raises
 `UnsupportedModel`.
 
-Width 384 (hac), the headline path (`forward_tiles`): activations tile-major `[tile][T][64][H]`, gate pre-activations
-`[tile][T][8][64][192]`; per layer ONE input GEMM over all tiles and ONE launch of the recurrent kernel (one 8-CTA
-cluster per 64-chunk tile, 8 clusters for 512 chunks), 15 launches per batch, issued by
-one C call (`b200_lstm_crf_fwd`) unless per-kernel events or intermediate activations are asked for.  Buffers are cached
-per (batch, chunk length, slot): `slot` selects one of several independent buffer sets, so that consecutive batches can
-be in flight on different streams (`score_batches`, bench.py).
+Every layout shares the front end: the fused conv1 + conv2 stem writes `[N][Lp][C2]` channels last, and the strided conv3 is
+one GEMM over the overlapping-row view of it.  The LSTM width picks one of three activation layouts (`LstmCrfPlan.forward`):
 
-Other widths (`forward_tiled`): the generic `[T][N][4H]` layout and the `mma.sync` recurrent kernel, tiles of 32 chunks
-pipelined on per-tile streams; `B200_LSTM_TILE=0` sends width 384 down this path (8-CTA clusters), `B200_TILE_STREAMS=1` gives the tile-layout path per-tile streams as well (the round-1 schedule).
+* Tile layout, width 384 (hac, the headline path; `forward_tiles`): activations tile-major `[tile][T][64][H]`, gate
+  pre-activations `[tile][T][8][64][192]`; layer by layer on the current stream, per layer ONE input GEMM over all tiles
+  and ONE launch of the wgmma recurrent kernel (one 8-CTA cluster per 64-chunk tile, 8 clusters for 512 chunks).  The
+  whole encoder is one C call (`b200_lstm_crf_fwd`) unless per-kernel events, intermediate activations, another GEMM
+  implementation or the int8 input projection ask for the launches one at a time.  Buffers are cached per (batch, chunk
+  length, slot): `slot` selects one of several independent buffer sets, so that consecutive batches can be in flight on
+  different streams (`score_batches`, bench.py).
 
-Widths 768 and 1024 (`forward_wide`: dna_r9.4.1@v3.1, dna_r10.4.1@v4.3): W_hh does not fit the shared memory of one cluster,
-so the recurrence runs on the grid-wide kernel (lstm_rec_wide.cu: H / 8 co-resident CTAs, one cooperative launch per layer);
-activations `[T][N][H]`, gate pre-activations `[T][H/8][N][32]`, layer by layer on the current stream, one buffer set (no
-slots), no int8 input projection; the output of the Linear in front of the head, if any, is `[T][N][B]`.
+* Generic layout, widths 96, 128 and 256, and 384 under `B200_LSTM_TILE=0` (`forward_generic`): the `mma.sync` recurrent
+  kernel on activations `[T][n][H]` and gate pre-activations `[T][n][4H]` of a tile of n chunks.  A batch of more than
+  one 32-chunk tile runs its tiles on streams of their own, so that the GEMMs of one tile fill the SMs the recurrences of
+  the others leave free; a single tile runs on the current stream.
+
+* Wide layout, widths 768 and 1024 (`forward_wide`: dna_r9.4.1@v3.1, dna_r10.4.1@v4.3): W_hh does not fit the shared memory
+  of one cluster, so the recurrence runs on the grid-wide kernel (lstm_rec_wide.cu: H / 8 co-resident CTAs, one cooperative
+  launch per layer); activations `[T][N][H]`, gate pre-activations `[T][H/8][N][32]`, layer by layer on the current
+  stream, one buffer set (no slots), no int8 input projection; the output of the Linear in front of the head, if any, is
+  `[T][N][B]`.
 """
+
+import os
+import threading
 
 import torch
 
@@ -118,30 +128,11 @@ def _dev16(t, device):
 
 
 class _Stage:
-    """Context manager recording a CUDA event pair around one kernel launch (no-op without a sink)."""
+    """Context manager recording a CUDA event pair around one kernel launch on `stream` (default: the current stream); no-op
+    without a sink."""
 
-    def __init__(self, name, sink):
-        self.name, self.sink = name, sink
-
-    def __enter__(self):
-        if self.sink is not None:
-            self.start = torch.cuda.Event(enable_timing=True)
-            self.start.record()
-
-    def __exit__(self, *exc):
-        if self.sink is not None:
-            end = torch.cuda.Event(enable_timing=True)
-            end.record()
-            self.sink.append((self.name, self.start, end))
-        return False
-
-
-class _StreamStage(_Stage):
-    """`_Stage` whose events are recorded on an explicit stream."""
-
-    def __init__(self, name, sink, stream):
-        super().__init__(name, sink)
-        self.stream = stream
+    def __init__(self, name, sink, stream=None):
+        self.name, self.sink, self.stream = name, sink, stream
 
     def __enter__(self):
         if self.sink is not None:
@@ -281,197 +272,153 @@ class LstmCrfPlan:
     def frames(self, L):
         return (L + 2 * self.pad3 - self.k3) // self.s3 + 1
 
-    def _buffers(self, N, L):
-        key = (N, L)
-        if key not in self._bufs:
-            self._bufs.clear()
-            T = self.frames(L)
-            need = max(self.pad3 + L, (T - 1) * self.s3 + self.k3)
-            Tp = -(-need // self.s3)
-            Lp = Tp * self.s3
-            dev, f16 = self.device, torch.float16
-            tail = self.k3 * self.c2  # the last window of the overlapping-row view reads past row N*Tp-1
-            self._bufs[key] = dict(
-                T=T, Tp=Tp, Lp=Lp,
-                stem=torch.empty(N * Lp * self.c2 + tail, dtype=f16, device=dev),
-                ya=torch.empty(T, N, self.hidden, dtype=f16, device=dev),
-                yb=torch.empty(T, N, self.hidden, dtype=f16, device=dev),
-                gx=torch.empty(T, N, 4 * self.hidden, dtype=f16, device=dev),
-            )
-            self._bufs[key]["stem"][-tail:].zero_()
-        return self._bufs[key]
-
     @property
     def supports_slots(self):
-        """Independent buffer sets (several batches in flight) exist for the tile-layout path only."""
-        import os
+        """Independent buffer sets (several batches in flight) exist for the tile layout only."""
         return bool(self.tile) and os.environ.get("B200_LSTM_TILE", "1") != "0"
 
-    TILE = 32  # chunks per recurrent cluster
-    # CTAs a per-tile GEMM may occupy while recurrent clusters of other tiles are resident (0 = all SMs)
-    TILE_GEMM_CTAS = 0
+    TILE = 32  # chunks per tile of the generic layout (one recurrent cluster each)
 
-    def _tile_buffers(self, N, L):
-        key = ("tiled", N, L)
-        if key not in self._bufs:
-            self._bufs.clear()
-            T = self.frames(L)
-            need = max(self.pad3 + L, (T - 1) * self.s3 + self.k3)
-            Tp = -(-need // self.s3)
-            Lp = Tp * self.s3
-            dev, f16, H = self.device, torch.float16, self.hidden
+    def _buffers(self, layout, N, L, slot=0):
+        """
+        Work buffers of `layout` ("generic", "tile" or "wide") for N chunks of L samples.  Buffer sets of another layout or
+        geometry are dropped; the slots of one layout and geometry stay side by side (batches in flight).
+        """
+        key = (layout, N, L, slot)
+        if key in self._bufs:
+            return self._bufs[key]
+        for k in [k for k in self._bufs if k[:3] != key[:3]]:
+            del self._bufs[k]
+        T = self.frames(L)
+        need = max(self.pad3 + L, (T - 1) * self.s3 + self.k3)
+        Tp = -(-need // self.s3)
+        Lp = Tp * self.s3
+        dev, f16, H = self.device, torch.float16, self.hidden
+        tail = self.k3 * self.c2  # the last window of the overlapping-row view reads past row N*Tp-1
+        b = dict(T=T, Tp=Tp, Lp=Lp, stem=torch.empty(N * Lp * self.c2 + tail, dtype=f16, device=dev))
+        b["stem"][-tail:].zero_()
+        if layout == "generic":
+            # flat: the tile of chunks [n0, n0 + nb) is [T][nb][.] at element n0*T*H of ya / yb (n0*T*4H of gx)
             nt = -(-N // self.TILE)
-            tail = self.k3 * self.c2
-            stem = torch.empty(N * Lp * self.c2 + tail, dtype=f16, device=dev)
-            stem[-tail:].zero_()
-            self._bufs[key] = dict(
-                T=T, Tp=Tp, Lp=Lp, nt=nt, stem=stem,
-                ya=torch.empty(nt, T, self.TILE, H, dtype=f16, device=dev),
-                yb=torch.empty(nt, T, self.TILE, H, dtype=f16, device=dev),
-                gx=torch.empty(nt, T, self.TILE, 4 * H, dtype=f16, device=dev),
-                streams=_LazyStreams(dev, nt), rec_streams=_LazyStreams(dev, nt),
-                rec_ready=[torch.cuda.Event() for _ in range(nt)], rec_done=[torch.cuda.Event() for _ in range(nt)],
-                done=[torch.cuda.Event() for _ in range(nt)],
-                head=[torch.cuda.Event() for _ in range(nt)],
-                start=torch.cuda.Event(),
+            b.update(ya=torch.empty(N * T * H, dtype=f16, device=dev), yb=torch.empty(N * T * H, dtype=f16, device=dev),
+                     gx=torch.empty(N * T * 4 * H, dtype=f16, device=dev),
+                     streams=_LazyStreams(dev, nt), start=torch.cuda.Event(), done=[torch.cuda.Event() for _ in range(nt)])
+        elif layout == "tile":
+            TB, CS = self.tile, self.tile_cs
+            nt = -(-N // TB)
+            b.update(
+                nt=nt,
+                # zero-filled once: rows of chunks beyond the batch (last tile) are never written and must stay finite
+                ya=torch.zeros(nt, T, TB, H, dtype=f16, device=dev),
+                yb=torch.zeros(nt, T, TB, H, dtype=f16, device=dev),
+                gx=torch.zeros(nt, T, CS, TB, 4 * H // CS, dtype=f16, device=dev),
+                yq=torch.empty(nt * T * TB * H, dtype=torch.int8, device=dev) if self.quantize else None,
+                # staging of the recurrent kernel's h all-gather: one region per tile (the clusters run concurrently)
+                hx=torch.empty(nt, native.lstm_rec_tile_workspace_bytes(TB), dtype=torch.uint8, device=dev),
             )
-        return self._bufs[key]
+        else:
+            ws = torch.empty(native.lstm_rec_wide_workspace_bytes(N, H), dtype=torch.uint8, device=dev)
+            off = native.lstm_rec_wide_status_offset(N, H)
+            b.update(
+                ya=torch.empty(T, N, H, dtype=f16, device=dev),
+                yb=torch.empty(T, N, H, dtype=f16, device=dev),
+                gx=torch.empty(T, self.wide, N, 4 * H // self.wide, dtype=f16, device=dev),
+                yl=None if self.wb is None else torch.empty(T, N, self.head_in, dtype=f16, device=dev),
+                ws=ws, ws_status=ws[off:off + 4].view(torch.int32),
+                status=torch.zeros(len(self.lstm), dtype=torch.int32, device=dev),
+            )
+        self._bufs[key] = b
+        return b
 
-    def forward_tiled(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, decode=None):
-        """
-        Tile-pipelined forward (see module docstring): same result as `forward(..., tiled=False)`.
-        `decode=(qscale, qbias)`: also enqueue the CRF decode of every tile on that tile's stream, right behind its
-        CRF GEMM (it then overlaps the recurrences of the other tiles); the results are parked in `DECODE_CACHE` and
-        handed out by `CrfDecoder` when it is asked to decode exactly these scores with exactly these parameters.
-        Off by default: measured 5 % slower end to end (34.9 vs 33.0 ms/step), the decode CTAs land on the SMs of
-        the recurrent clusters and lengthen their per-step critical path.
-        """
+    # ------------------------------------------------------------------------------------------
+    # front end, shared by the three layouts
+    # ------------------------------------------------------------------------------------------
+    def _input(self, x):
+        """[N, 1, L] or [N, L] -> contiguous fp16 [N, L] on the plan's device."""
         if x.dim() == 3:
             x = x[:, 0, :]
-        x = x.to(device=self.device, dtype=torch.float16).contiguous()
+        return x.to(device=self.device, dtype=torch.float16).contiguous()
+
+    def _stem(self, x, b, events, feats):
+        """conv1 + conv2 into b["stem"] ([N][Lp][C2], channels last); `feats` (a dict or None) gets the "stem" activations."""
+        N, L = x.shape
+        Lp = b["Lp"]
+        with _Stage("conv_stem", events):
+            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3,
+                             bounds=self.stem_bounds)
+        if feats is not None:
+            feats["stem"] = b["stem"][:N * Lp * self.c2].view(N, Lp, self.c2)[:, self.pad3:self.pad3 + L].clone()
+
+    def _conv_gemm(self, b, n0, nb, dst, events, gemm_impl, stream=None, **rows):
+        """The strided conv of chunks [n0, n0 + nb) as one GEMM: rows r = n*Tp + t are windows of k3*c2 stem elements, s3*c2
+        apart; `rows` maps them into `dst` (b200_gemm_fwd_ex)."""
+        with _Stage("conv_gemm", events, stream):
+            native.gemm(b["stem"][n0 * b["Lp"] * self.c2:], self.s3 * self.c2, self.w3, self.b3, dst, self.hidden,
+                        nb * b["Tp"], self.hidden, self.k3 * self.c2, act=self.act3, lo=self.lo3, hi=self.hi3,
+                        rows_inner=b["Tp"], valid_inner=b["T"], stride_outer=1, impl=gemm_impl, stream=stream, **rows)
+
+    # ------------------------------------------------------------------------------------------
+    # generic layout: tiles of n chunks, activations [T][n][H], gate pre-activations [T][n][4H]
+    # ------------------------------------------------------------------------------------------
+    def forward_generic(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, return_features=False, tiled=None):
+        """
+        Forward in the generic layout.  `tiled` (default: when the batch has more than one tile): 32-chunk tiles, each on a
+        stream of its own and all started behind the stem; otherwise the batch is one tile on the current stream.
+        Intermediate activations (`return_features`) are taken from the single-tile schedule.
+        """
+        x = self._input(x)
         N, L = x.shape
         H, TB = self.hidden, self.TILE
-        b = self._tile_buffers(N, L)
-        T, Tp, Lp, nt = b["T"], b["Tp"], b["Lp"], b["nt"]
+        b = self._buffers("generic", N, L)
+        T = b["T"]
         if out is None:
             out = torch.empty(N, T, self.n_scores, dtype=torch.float16, device=self.device)
-        main = torch.cuda.current_stream()
-        dec = None
-        if decode is not None:
-            ws_tile = native.crf_decode_workspace_bytes(TB, T, self.state_len)
-            if b.get("dec_ws") is None or b["dec_ws"].numel() < ws_tile * nt:
-                b["dec_ws"] = torch.empty(ws_tile * nt, dtype=torch.uint8, device=self.device)
-            dec = [torch.empty(N, T, dtype=torch.uint8, device=self.device) for _ in range(3)]  # moves, seq, qual
+        feats = {} if return_features else None
+        tiled = (N > TB if tiled is None else tiled) and not return_features
+        tiles = [(n0, min(TB, N - n0), b["streams"][n0 // TB]) for n0 in range(0, N, TB)] if tiled else [(0, N, None)]
 
-        with _Stage("conv_stem", events):
-            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3)
-        tiles = []
-        for i in range(nt):
-            n0 = i * TB
-            nb = min(TB, N - n0)
-            tiles.append((i, n0, nb, b["streams"][i]))
+        def in_gemm(src, layer, n0, nb, st):
+            with _Stage("lstm_in_gemm", events, st):
+                native.gemm(src[n0 * T * H:], H, layer["wih"], layer["bias"], b["gx"][n0 * T * 4 * H:], 4 * H, T * nb, 4 * H,
+                            H, impl=gemm_impl, stream=st)
 
-        def staged(name, st):
-            return _StreamStage(name, events, st)
-
-        import os
-        cap = int(os.environ.get("B200_TILE_GEMM_CTAS", self.TILE_GEMM_CTAS))
-        stagger = os.environ.get("B200_TILE_STAGGER", "0") != "0"
-        rec_prio = os.environ.get("B200_LSTM_PRIO", "1") != "0"   # recurrent kernels on high-priority side streams
-
-        # Head of the pipeline.  With every tile's first GEMMs on its own stream they share the machine and finish
-        # together; the 15 cluster slots then fill and drain in lock-step and the GEMMs of the next layer again arrive
-        # all at once (measured: 4.2 ms per layer = 1.2 ms GEMM phase + 2.5 ms recurrence + the 16th tile trailing).
-        # B200_TILE_STAGGER=1 serialises the head GEMMs on the main stream so that the tiles stay staggered; measured
-        # slightly slower (29.4 vs 28.8 ms/step): persistent GEMM CTAs then squat on SMs a waiting cluster needs, and
-        # every recurrent launch queues ~0.9 ms for 8 free SMs inside one GPC.  Lock-step is the default.
-        # The recurrent kernels go to a HIGH-PRIORITY side stream per tile (B200_LSTM_PRIO=0 turns that off): when SMs free
-        # up, a waiting cluster is placed before the queued CTAs of the other tiles' GEMMs (24.2 -> 22.9 ms/step).
-        first = self.lstm[0]
-        for i, n0, nb, st in tiles:
-            head = main if stagger else st
-            if not stagger and i == 0:
-                b["start"].record(main)
-            if not stagger:
+        self._stem(x, b, events, feats)
+        if tiled:
+            b["start"].record()
+        for n0, nb, st in tiles:    # every tile's conv GEMM and first input GEMM are enqueued ahead of any recurrence
+            if tiled:
                 st.wait_event(b["start"])
-            with staged("conv_gemm", head):   # rows r = i_chunk*Tp + t of this tile -> ya[tile][t][i_chunk]
-                native.gemm(b["stem"][n0 * Lp * self.c2:], self.s3 * self.c2, self.w3, self.b3, b["ya"][i], H, nb * Tp, H,
-                            self.k3 * self.c2, act=self.act3, rows_inner=Tp, valid_inner=T, stride_inner=nb,
-                            stride_outer=1, impl=gemm_impl, stream=head)
-            with staged("lstm_in_gemm", head):
-                native.gemm(b["ya"][i], H, first["wih"], first["bias"], b["gx"][i], 4 * H, T * nb, 4 * H, H,
-                            impl=gemm_impl, stream=head)
-            if stagger:
-                b["head"][i].record(main)
-                st.wait_event(b["head"][i])
+            self._conv_gemm(b, n0, nb, b["ya"][n0 * T * H:], events, gemm_impl, st, stride_inner=nb)
+            if feats is not None:
+                feats["conv"] = b["ya"].view(T, N, H).clone()
+            in_gemm(b["ya"], self.lstm[0], n0, nb, st)
         cur, nxt = b["ya"], b["yb"]
         for li, layer in enumerate(self.lstm):
-            for i, n0, nb, st in tiles:
+            for n0, nb, st in tiles:
                 if li > 0:
-                    with staged("lstm_in_gemm", st):
-                        native.gemm(cur[i], H, layer["wih"], layer["bias"], b["gx"][i], 4 * H, T * nb, 4 * H, H,
-                                    impl=gemm_impl, stream=st, max_ctas=cap)
-                if rec_prio:
-                    rs = b["rec_streams"][i]
-                    b["rec_ready"][i].record(st)
-                    rs.wait_event(b["rec_ready"][i])
-                    with staged("lstm_rec", rs):
-                        native.lstm_rec(b["gx"][i], layer["whh"], nxt[i], T, nb, H, layer["reverse"], stream=rs)
-                    b["rec_done"][i].record(rs)
-                    st.wait_event(b["rec_done"][i])
-                else:
-                    with staged("lstm_rec", st):
-                        native.lstm_rec(b["gx"][i], layer["whh"], nxt[i], T, nb, H, layer["reverse"], stream=st)
+                    in_gemm(cur, layer, n0, nb, st)
+                with _Stage("lstm_rec", events, st):
+                    native.lstm_rec(b["gx"][n0 * T * 4 * H:], layer["whh"], nxt[n0 * T * H:], T, nb, H, layer["reverse"],
+                                    stream=st)
             cur, nxt = nxt, cur
-        for i, n0, nb, st in tiles:
-            with staged("crf_gemm", st):    # rows r = t*nb + i_chunk -> out[n0 + i_chunk][t]
-                native.gemm(cur[i], H, self.wl, self.bl, out[n0:], self.n_scores, T * nb, self.n_scores, H,
+            if feats is not None:
+                feats[f"lstm{li}"] = cur.view(T, N, H).clone()
+        for i, (n0, nb, st) in enumerate(tiles):
+            with _Stage("crf_gemm", events, st):    # rows r = t*nb + i_chunk -> out[n0 + i_chunk][t]
+                native.gemm(cur[n0 * T * H:], H, self.wl, self.bl, out[n0:], self.n_scores, T * nb, self.n_scores, H,
                             act=self.act_l, lo=self.lo, hi=self.hi, rows_inner=nb, valid_inner=nb, stride_inner=T,
-                            stride_outer=1, impl=gemm_impl, stream=st, max_ctas=cap)
-            if dec is not None:
-                with staged("crf_decode", st):
-                    native.crf_decode(out[n0:n0 + nb], self.state_len, self.blank_score, decode[0], decode[1],
-                                      b["dec_ws"][i * ws_tile:], dec[0][n0:], dec[1][n0:], dec[2][n0:], stream=st)
-            b["done"][i].record(st)
-        for i in range(nt):
-            main.wait_event(b["done"][i])
-        if dec is not None:
-            DECODE_CACHE.put(out, (self.state_len, self.blank_score, float(decode[0]), float(decode[1])), tuple(dec))
-        return out
+                            stride_outer=1, impl=gemm_impl, stream=st)
+            if tiled:
+                b["done"][i].record(st)
+        if tiled:
+            main = torch.cuda.current_stream()
+            for done in b["done"]:
+                main.wait_event(done)
+        return (out, feats) if return_features else out
 
     # ------------------------------------------------------------------------------------------
     # tile layout (H = 384): activations [tile][T][64][H], gate pre-activations [tile][T][8][64][192]
     # ------------------------------------------------------------------------------------------
-    def _tile_layout_buffers(self, N, L, slot=0):
-        key = ("tiles", N, L, slot)
-        if key not in self._bufs:
-            for k in [k for k in self._bufs if k[0] != "tiles" or k[1:3] != (N, L)]:
-                del self._bufs[k]
-            T = self.frames(L)
-            need = max(self.pad3 + L, (T - 1) * self.s3 + self.k3)
-            Tp = -(-need // self.s3)
-            Lp = Tp * self.s3
-            dev, f16, H, TB = self.device, torch.float16, self.hidden, self.tile
-            nt = -(-N // TB)
-            tail = self.k3 * self.c2
-            stem = torch.empty(N * Lp * self.c2 + tail, dtype=f16, device=dev)
-            stem[-tail:].zero_()
-            self._bufs[key] = dict(
-                T=T, Tp=Tp, Lp=Lp, nt=nt, stem=stem,
-                # zero-filled once: rows of chunks beyond the batch (last tile) are never written and must stay finite
-                ya=torch.zeros(nt, T, TB, H, dtype=f16, device=dev),
-                yb=torch.zeros(nt, T, TB, H, dtype=f16, device=dev),
-                gx=torch.zeros(nt, T, self.tile_cs, TB, 4 * H // self.tile_cs, dtype=f16, device=dev),
-                yq=torch.empty(nt * T * TB * H, dtype=torch.int8, device=dev) if self.quantize else None,
-                # staging of the recurrent kernel's h all-gather: one region per tile (tiles run concurrently)
-                hx=torch.empty(nt, native.lstm_rec_tile_workspace_bytes(TB), dtype=torch.uint8, device=dev),
-                streams=_LazyStreams(dev, nt), rec_streams=_LazyStreams(dev, nt),
-                rec_ready=[torch.cuda.Event() for _ in range(nt)], rec_done=[torch.cuda.Event() for _ in range(nt)],
-                done=[torch.cuda.Event() for _ in range(nt)],
-                start=torch.cuda.Event(),
-            )
-        return self._bufs[key]
-
     def _plan_struct(self, b, N, L):
         """`b200_lstm_crf_plan` for this geometry and buffer set (cached in the buffer dict)."""
         if "struct" not in b:
@@ -492,170 +439,73 @@ class LstmCrfPlan:
             b["struct"] = p
         return b["struct"]
 
-    def forward_tiles(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, return_features=False, streams=False,
-                      slot=0):
+    def forward_tiles(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, return_features=False, slot=0):
         """
-        Forward in the tile layout.  `streams=False`: layer by layer on the current stream -- one input-projection GEMM
-        and ONE recurrent launch (a cluster per tile, all in one wave) per layer.  `streams=True`: every tile gets its own
-        stream (conv GEMM -> 5 x (input GEMM -> recurrent cluster) -> CRF GEMM), recurrent launches on high-priority side
-        streams, so the GEMMs of one tile fill the SMs the other tiles' clusters leave free.  Bit-identical results.
-        `slot` selects one of several independent buffer sets (batches in flight at the same time).
+        Forward in the tile layout, layer by layer on the current stream: one input-projection GEMM and ONE recurrent launch
+        (a cluster per tile, all in one wave) per layer.  `slot` selects one of several independent buffer sets (batches in
+        flight at the same time).
         """
-        import os
-        if x.dim() == 3:
-            x = x[:, 0, :]
-        x = x.to(device=self.device, dtype=torch.float16).contiguous()
+        x = self._input(x)
         N, L = x.shape
         H, TB, CS = self.hidden, self.tile, self.tile_cs
         CW = 4 * H // CS                     # gx columns per cluster rank (192)
-        b = self._tile_layout_buffers(N, L, slot)
-        T, Tp, Lp, nt = b["T"], b["Tp"], b["Lp"], b["nt"]
+        b = self._buffers("tile", N, L, slot)
+        T, nt = b["T"], b["nt"]
         if out is None:
             out = torch.empty(N, T, self.n_scores, dtype=torch.float16, device=self.device)
-        main = torch.cuda.current_stream()
-        feats = {}
-        cap = int(os.environ.get("B200_TILE_GEMM_CTAS", self.TILE_GEMM_CTAS))
-
-        def staged(name, st):
-            return _StreamStage(name, events, st)
-
-        def conv_gemm(i, st):       # rows r = i_chunk*Tp + t of tile i -> ya[i][t][i_chunk]
-            n0 = i * TB
-            nb = min(TB, N - n0)
-            with staged("conv_gemm", st):
-                native.gemm(b["stem"][n0 * Lp * self.c2:], self.s3 * self.c2, self.w3, self.b3, b["ya"][i], H, nb * Tp, H,
-                            self.k3 * self.c2, act=self.act3, rows_inner=Tp, valid_inner=T, stride_inner=TB,
-                            stride_outer=1, impl=gemm_impl, stream=st)
-
-        def in_gemm(src, layer, tiles, st, max_ctas=0):      # rows (tile, t, chunk) -> gx[tile][t][rank][chunk][CW]
-            i0, cnt = tiles
-            if self.quantize:
-                rows = cnt * T * TB
-                yq = b["yq"][i0 * T * TB * H:]
-                with staged("quantize_i8", st):
-                    native.quantize_i8(src[i0:i0 + cnt], yq[:rows * H], 127.0, stream=st)
-                with staged("lstm_in_gemm", st):
-                    native.gemm_i8(yq, H, layer["wih_q"], layer["wih_scale"], layer["bias"], b["gx"][i0], CW, rows, 4 * H, H,
-                                   rows_inner=TB, valid_inner=TB, stride_inner=1, stride_outer=CS * TB, cb_width=CW,
-                                   cb_rows=TB, stream=st, max_ctas=max_ctas)
-                return
-            with staged("lstm_in_gemm", st):
-                native.gemm(src[i0], H, layer["wih"], layer["bias"], b["gx"][i0], CW, cnt * T * TB, 4 * H, H,
-                            rows_inner=TB, valid_inner=TB, stride_inner=1, stride_outer=CS * TB, cb_width=CW, cb_rows=TB,
-                            impl=gemm_impl, stream=st, max_ctas=max_ctas)
-
-        def rec(dst, layer, tiles, st):
-            i0, cnt = tiles
-            n = min(cnt * TB, N - i0 * TB)
-            with staged("lstm_rec", st):
-                native.lstm_rec_tile(b["gx"][i0], layer["whh"], dst[i0], T, n, H, layer["reverse"], stream=st,
-                                     workspace=b["hx"][i0])
-
-        def crf_gemm(src, i, st, max_ctas=0):   # rows r = t*TB + i_chunk of tile i -> out[n0 + i_chunk][t]
-            n0 = i * TB
-            nb = min(TB, N - n0)
-            with staged("crf_gemm", st):
-                native.gemm(src[i], H, self.wl, self.bl, out[n0:], self.n_scores, T * TB, self.n_scores, H,
-                            act=self.act_l, lo=self.lo, hi=self.hi, rows_inner=TB, valid_inner=nb, stride_inner=T,
-                            stride_outer=1, impl=gemm_impl, stream=st, max_ctas=max_ctas)
+        if events is None and not return_features and gemm_impl == native.GEMM_AUTO and not self.quantize \
+                and len(self.lstm) <= native.MAX_LSTM_LAYERS:
+            # the whole encoder from ONE C-ABI call (b200_lstm_crf_fwd); the per-kernel path below runs the same launches
+            # one ctypes call at a time (used when per-kernel events or intermediate activations are wanted)
+            native.lstm_crf_fwd(self._plan_struct(b, N, L), x, out)
+            return out
 
         def gather(buf):            # [tile][T][64][H] -> [T][N][H]
             return buf.permute(1, 0, 2, 3).reshape(T, nt * TB, H)[:, :N].clone()
 
-        if not streams and events is None and not return_features and gemm_impl == native.GEMM_AUTO and not self.quantize \
-                and len(self.lstm) <= native.MAX_LSTM_LAYERS and os.environ.get("B200_COARSE_FWD", "1") != "0":
-            # the whole encoder from ONE C-ABI call (b200_lstm_crf_fwd); the per-kernel path below runs the same launches
-            # one ctypes call at a time (used when per-kernel events or intermediate activations are wanted)
-            native.lstm_crf_fwd(self._plan_struct(b, N, L), x, out, stream=main)
-            return out
-
-        with _StreamStage("conv_stem", events, main):
-            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3)
-        if return_features:
-            feats["stem"] = b["stem"][:N * Lp * self.c2].view(N, Lp, self.c2)[:, self.pad3:self.pad3 + L].clone()
+        feats = {} if return_features else None
+        self._stem(x, b, events, feats)
+        # all tiles in one launch: chunk n of the stem -> (tile n / TB, row n % TB)
+        self._conv_gemm(b, 0, N, b["ya"], events, gemm_impl, stride_inner=TB, group=TB, stride_group=T * TB)
         cur, nxt = b["ya"], b["yb"]
-
-        if not streams:
-            # all tiles in one launch: chunk n of the stem -> (tile n / TB, row n % TB); rows r = n*Tp + t
-            with staged("conv_gemm", main):
-                native.gemm(b["stem"], self.s3 * self.c2, self.w3, self.b3, b["ya"], H, N * Tp, H, self.k3 * self.c2,
-                            act=self.act3, rows_inner=Tp, valid_inner=T, stride_inner=TB, stride_outer=1, group=TB,
-                            stride_group=T * TB, impl=gemm_impl, stream=main)
-            if return_features:
-                feats["conv"] = gather(cur)
-            for li, layer in enumerate(self.lstm):
-                in_gemm(cur, layer, (0, nt), main)
-                rec(nxt, layer, (0, nt), main)
-                cur, nxt = nxt, cur
-                if return_features:
-                    feats[f"lstm{li}"] = gather(cur)
-            # all tiles in one launch: rows r = (tile*T + t)*TB + i -> out[tile*TB + i][t]; rows of chunks beyond the batch
-            # (last tile) land behind the N valid chunks and are cut off by `valid_rows`
-            if N % TB == 0:
-                with staged("crf_gemm", main):
-                    native.gemm(cur, H, self.wl, self.bl, out, self.n_scores, nt * T * TB, self.n_scores, H, act=self.act_l,
-                                lo=self.lo, hi=self.hi, rows_inner=TB, valid_inner=TB, stride_inner=T, stride_outer=1,
-                                group=T, stride_group=TB * T, impl=gemm_impl, stream=main)
-            else:
-                full = N // TB
-                if full:
-                    with staged("crf_gemm", main):
-                        native.gemm(cur, H, self.wl, self.bl, out, self.n_scores, full * T * TB, self.n_scores, H,
-                                    act=self.act_l, lo=self.lo, hi=self.hi, rows_inner=TB, valid_inner=TB, stride_inner=T,
-                                    stride_outer=1, group=T, stride_group=TB * T, impl=gemm_impl, stream=main)
-                crf_gemm(cur, nt - 1, main)
-            return (out, feats) if return_features else out
-
-        b["start"].record(main)
-        for i in range(nt):
-            st = b["streams"][i]
-            st.wait_event(b["start"])
-            conv_gemm(i, st)
+        if feats is not None:
+            feats["conv"] = gather(cur)
+        rows = dict(rows_inner=TB, valid_inner=TB, stride_inner=1, stride_outer=CS * TB, cb_width=CW, cb_rows=TB)
         for li, layer in enumerate(self.lstm):
-            for i in range(nt):
-                st, rs = b["streams"][i], b["rec_streams"][i]
-                in_gemm(cur, layer, (i, 1), st, max_ctas=cap if li > 0 else 0)
-                b["rec_ready"][i].record(st)
-                rs.wait_event(b["rec_ready"][i])
-                rec(nxt, layer, (i, 1), rs)
-                b["rec_done"][i].record(rs)
-                st.wait_event(b["rec_done"][i])
+            # rows (tile, t, chunk) -> gx[tile][t][rank][chunk][CW]
+            if self.quantize:
+                with _Stage("quantize_i8", events):
+                    native.quantize_i8(cur, b["yq"], 127.0)
+                with _Stage("lstm_in_gemm", events):
+                    native.gemm_i8(b["yq"], H, layer["wih_q"], layer["wih_scale"], layer["bias"], b["gx"], CW, nt * T * TB,
+                                   4 * H, H, **rows)
+            else:
+                with _Stage("lstm_in_gemm", events):
+                    native.gemm(cur, H, layer["wih"], layer["bias"], b["gx"], CW, nt * T * TB, 4 * H, H, impl=gemm_impl,
+                                **rows)
+            with _Stage("lstm_rec", events):
+                native.lstm_rec_tile(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"], workspace=b["hx"])
             cur, nxt = nxt, cur
-        for i in range(nt):
-            st = b["streams"][i]
-            crf_gemm(cur, i, st, max_ctas=cap)
-            b["done"][i].record(st)
-            main.wait_event(b["done"][i])
-        return out
+            if feats is not None:
+                feats[f"lstm{li}"] = gather(cur)
+        # full tiles in one launch: rows r = (tile*T + t)*TB + i -> out[tile*TB + i][t]; a last tile the batch does not fill
+        # in a launch of its own, whose `valid_inner` cuts off the rows of chunks beyond the batch
+        full = N // TB
+        if full:
+            with _Stage("crf_gemm", events):
+                native.gemm(cur, H, self.wl, self.bl, out, self.n_scores, full * T * TB, self.n_scores, H, act=self.act_l,
+                            lo=self.lo, hi=self.hi, rows_inner=TB, valid_inner=TB, stride_inner=T, stride_outer=1,
+                            group=T, stride_group=TB * T, impl=gemm_impl)
+        if N % TB:
+            with _Stage("crf_gemm", events):
+                native.gemm(cur[full], H, self.wl, self.bl, out[full * TB:], self.n_scores, T * TB, self.n_scores, H,
+                            act=self.act_l, lo=self.lo, hi=self.hi, rows_inner=TB, valid_inner=N - full * TB,
+                            stride_inner=T, stride_outer=1, impl=gemm_impl)
+        return (out, feats) if return_features else out
 
     # ------------------------------------------------------------------------------------------
-    # wide widths (H = 768, 1024): activations [T][N][H], gate pre-activations [T][G][N][32], one grid-wide recurrent launch
+    # wide layout (H = 768, 1024): activations [T][N][H], gate pre-activations [T][G][N][32], one grid-wide recurrent launch
     # ------------------------------------------------------------------------------------------
-    def _wide_buffers(self, N, L):
-        key = ("wide", N, L)
-        if key not in self._bufs:
-            self._bufs.clear()
-            T = self.frames(L)
-            need = max(self.pad3 + L, (T - 1) * self.s3 + self.k3)
-            Tp = -(-need // self.s3)
-            Lp = Tp * self.s3
-            dev, f16, H = self.device, torch.float16, self.hidden
-            tail = self.k3 * self.c2
-            ws = torch.empty(native.lstm_rec_wide_workspace_bytes(N, H), dtype=torch.uint8, device=dev)
-            off = native.lstm_rec_wide_status_offset(N, H)
-            self._bufs[key] = dict(
-                T=T, Tp=Tp, Lp=Lp,
-                stem=torch.empty(N * Lp * self.c2 + tail, dtype=f16, device=dev),
-                ya=torch.empty(T, N, H, dtype=f16, device=dev),
-                yb=torch.empty(T, N, H, dtype=f16, device=dev),
-                gx=torch.empty(T, self.wide, N, 4 * H // self.wide, dtype=f16, device=dev),
-                yl=None if self.wb is None else torch.empty(T, N, self.head_in, dtype=f16, device=dev),
-                ws=ws, ws_status=ws[off:off + 4].view(torch.int32),
-                status=torch.zeros(len(self.lstm), dtype=torch.int32, device=dev),
-            )
-            self._bufs[key]["stem"][-tail:].zero_()
-        return self._bufs[key]
-
     def _check_wide_status(self):
         """Raise if a recurrent launch of the previous wide-path forward gave up waiting for its peer CTAs."""
         pending, self._wide_pending = self._wide_pending, None
@@ -675,9 +525,7 @@ class LstmCrfPlan:
         (b200_lstm_wide_max_chunks) run as consecutive sub-batches.
         """
         self._check_wide_status()
-        if x.dim() == 3:
-            x = x[:, 0, :]
-        x = x.to(device=self.device, dtype=torch.float16).contiguous()
+        x = self._input(x)
         N, L = x.shape
         H, G = self.hidden, self.wide
         CW = 4 * H // G                     # gx columns per CTA (32)
@@ -690,24 +538,17 @@ class LstmCrfPlan:
             for n0 in range(0, N, cap):
                 self.forward_wide(x[n0:n0 + cap], out=out[n0:n0 + cap], gemm_impl=gemm_impl, events=events)
             return out
-        b = self._wide_buffers(N, L)
-        T, Tp, Lp = b["T"], b["Tp"], b["Lp"]
-        feats = {}
+        b = self._buffers("wide", N, L)
+        T = b["T"]
+        feats = {} if return_features else None
 
         def stage(name):
             return _Stage(name, events)
 
-        with stage("conv_stem"):
-            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3,
-                             bounds=self.stem_bounds)
-        if return_features:
-            feats["stem"] = b["stem"][:N * Lp * self.c2].view(N, Lp, self.c2)[:, self.pad3:self.pad3 + L].clone()
+        self._stem(x, b, events, feats)
         cur, nxt = b["ya"], b["yb"]
-        with stage("conv_gemm"):
-            native.gemm(b["stem"], self.s3 * self.c2, self.w3, self.b3, cur, H, N * Tp, H, self.k3 * self.c2,
-                        act=self.act3, lo=self.lo3, hi=self.hi3, rows_inner=Tp, valid_inner=T, stride_inner=N, stride_outer=1,
-                        impl=gemm_impl)
-        if return_features:
+        self._conv_gemm(b, 0, N, cur, events, gemm_impl, stride_inner=N)
+        if feats is not None:
             feats["conv"] = cur.clone()
         for i, layer in enumerate(self.lstm):
             with stage("lstm_in_gemm"):     # rows r = t*N + n -> gx[t][g][n][:], column block g = units [8g, 8g + 8)
@@ -717,13 +558,13 @@ class LstmCrfPlan:
                 native.lstm_rec_wide(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"], workspace=b["ws"])
             b["status"][i:i + 1].copy_(b["ws_status"])
             cur, nxt = nxt, cur
-            if return_features:
+            if feats is not None:
                 feats[f"lstm{i}"] = cur.clone()
         if self.wb is not None:
             with stage("bottleneck_gemm"):  # rows r = t*N + n -> yl[t][n][:]
                 native.gemm(cur, H, self.wb, self.bb, b["yl"], self.head_in, T * N, self.head_in, H, impl=gemm_impl)
             cur = b["yl"]
-            if return_features:
+            if feats is not None:
                 feats["linear"] = cur.clone()
 
         if out is None:
@@ -739,112 +580,30 @@ class LstmCrfPlan:
         self._wide_pending = (done, status)
         return (out, feats) if return_features else out
 
-    def forward(self, x, out=None, gemm_impl=native.GEMM_AUTO, return_features=False, events=None, tiled=None,
-                decode=None, slot=0):
-        with torch.cuda.device(self.device):    # streams / events / launches belong to the plan's device, whatever is current
-            return self._forward(x, out=out, gemm_impl=gemm_impl, return_features=return_features, events=events,
-                                 tiled=tiled, decode=decode, slot=slot)
-
-    def _forward(self, x, out=None, gemm_impl=native.GEMM_AUTO, return_features=False, events=None, tiled=None,
-                 decode=None, slot=0):
+    # ------------------------------------------------------------------------------------------
+    def forward(self, x, out=None, gemm_impl=native.GEMM_AUTO, return_features=False, events=None, tiled=None, slot=0):
         """
-        x: [N, 1, L] (or [N, L]) fp16 CUDA -> scores [N, T, C] fp16 (no blank column).
+        x: [N, 1, L] (or [N, L]) fp16 CUDA -> scores [N, T, C] fp16 (no blank column); with `return_features`, the pair
+        (scores, dict of intermediate activations).
         `events`: optional list; (stage, start, end) CUDA events are appended per kernel.
-        `tiled`: run the tile-pipelined schedule (default: whenever the batch has more than one 32-chunk tile).
-        `decode`: see `forward_tiled` (ignored by the single-stream schedule).
+        `tiled`: the schedule of the generic layout (see `forward_generic`); the tile and wide layouts have one schedule
+        each and ignore it.
+        `slot`: the buffer set of the tile layout (see `forward_tiles`); the other layouts have only slot 0.
         """
-        import os
-        if self.tile and os.environ.get("B200_LSTM_TILE", "1") != "0":
-            if tiled is None:
-                # Default: the layer-by-layer schedule (14 launches per batch).  With two batches in flight on two streams
-                # (score_batches, bench.py) it measured faster than per-tile streams on an H100 80GB HBM3 at 700 W (bench.py
-                # hac step, two 512-chunk batches in flight: 62.2 / 62.7 ms, one repeat at 73.7 ms, vs 66.1 / 66.1 ms):
-                # the GEMMs / decode of one batch fill the SMs the other batch's recurrent clusters leave free.
-                tiled = (not return_features) and x.shape[0] > self.tile and os.environ.get("B200_TILE_STREAMS", "0") != "0"
-            return self.forward_tiles(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features,
-                                      streams=tiled, slot=slot)
-        if slot != 0:
-            raise NotImplementedError("several batches in flight (slot != 0) need the tile-layout path (hidden size 384)")
-        if self.wide:
-            return self.forward_wide(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features)
-        if tiled is None:
-            tiled = (not return_features) and x.shape[0] > self.TILE
-        if tiled:
-            return self.forward_tiled(x, out=out, gemm_impl=gemm_impl, events=events, decode=decode)
-
-        def stage(name):
-            return _Stage(name, events)
-
-        if x.dim() == 3:
-            x = x[:, 0, :]
-        x = x.to(device=self.device, dtype=torch.float16).contiguous()
-        N, L = x.shape
-        H = self.hidden
-        b = self._buffers(N, L)
-        T, Tp, Lp = b["T"], b["Tp"], b["Lp"]
-        feats = {}
-
-        with stage("conv_stem"):
-            native.conv_stem(x, self.w1, self.b1, self.act1, self.w2, self.b2, self.act2, b["stem"], Lp, self.pad3)
-        if return_features:
-            feats["stem"] = b["stem"][:N * Lp * self.c2].view(N, Lp, self.c2)[:, self.pad3:self.pad3 + L].clone()
-
-        # strided conv: rows r = n*Tp + t are windows of k3*c2 elements, s3*c2 apart; out[t][n][:]
-        cur, nxt = b["ya"], b["yb"]
-        with stage("conv_gemm"):
-            native.gemm(b["stem"], self.s3 * self.c2, self.w3, self.b3, cur, H, N * Tp, H, self.k3 * self.c2,
-                        act=self.act3, rows_inner=Tp, valid_inner=T, stride_inner=N, stride_outer=1, impl=gemm_impl)
-        if return_features:
-            feats["conv"] = cur.clone()
-
-        for i, layer in enumerate(self.lstm):
-            with stage("lstm_in_gemm"):
-                native.gemm(cur, H, layer["wih"], layer["bias"], b["gx"], 4 * H, T * N, 4 * H, H, impl=gemm_impl)
-            with stage("lstm_rec"):
-                native.lstm_rec(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"])
-            cur, nxt = nxt, cur
-            if return_features:
-                feats[f"lstm{i}"] = cur.clone()
-
-        if out is None:
-            out = torch.empty(N, T, self.n_scores, dtype=torch.float16, device=self.device)
-        # rows r = t*N + n -> out[n][t][:]
-        with stage("crf_gemm"):
-            native.gemm(cur, H, self.wl, self.bl, out, self.n_scores, T * N, self.n_scores, H,
-                        act=self.act_l, lo=self.lo, hi=self.hi,
-                        rows_inner=N, valid_inner=N, stride_inner=T, stride_outer=1, impl=gemm_impl)
-        return (out, feats) if return_features else out
-
-
-class _DecodeCache:
-    """Decode results the tile-pipelined forward produced ahead of the `beam_search` call that will ask for them."""
-
-    def __init__(self):
-        self._entry = None
-
-    @staticmethod
-    def _version(t):
-        try:
-            return t._version
-        except RuntimeError:  # inference tensors carry no version counter
-            return -1
-
-    def put(self, scores, params, outputs):
-        self._entry = (scores.data_ptr(), tuple(scores.shape), self._version(scores), params, outputs)
-
-    def take(self, scores, params):
-        e, self._entry = self._entry, None
-        if e is not None and e[0] == scores.data_ptr() and e[1] == tuple(scores.shape) \
-                and e[2] == self._version(scores) and e[3] == params:
-            return e[4]
-        return None
-
-
-DECODE_CACHE = _DecodeCache()
+        with torch.cuda.device(self.device):    # streams / events / launches belong to the plan's device, whatever is current
+            if self.supports_slots:
+                return self.forward_tiles(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features,
+                                          slot=slot)
+            if slot != 0:
+                raise NotImplementedError("several batches in flight (slot != 0) need the tile-layout path (hidden size 384)")
+            if self.wide:
+                return self.forward_wide(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features)
+            return self.forward_generic(x, out=out, gemm_impl=gemm_impl, events=events, return_features=return_features,
+                                        tiled=tiled)
 
 
 class _LazyStreams:
-    """Per-tile streams of the tile-pipelined schedules, created on first use with `native.new_stream` (CUDA streams of their
+    """Per-tile streams of the generic layout, created on first use with `native.new_stream` (CUDA streams of their
     own).  `torch.cuda.Stream()` hands out streams from a pool of 32 per device round-robin: the 22 per-tile streams of two buffer
     sets, created eagerly, pushed later requests (the slot and copy streams of `score_batches`) onto pool entries already in use
     -- two "different" streams were then one CUDA stream and batches meant to overlap ran back to back (end-to-end step 17 ->
@@ -899,16 +658,8 @@ class CrfDecoder:
         if learned and beam is not None:
             raise ValueError("the beam search kernel needs a fixed blank score; scores with learned blank scores "
                              "(5 * 4**state_len columns) decode with the exact decoder only")
-        cached = None if learned else DECODE_CACHE.take(scores, (state_len, float(blank_score), float(qscale), float(qbias)))
-        if cached is not None:
-            if out is not None:
-                for dst, src in zip(out, cached):
-                    dst.copy_(src)
-                return tuple(out)
-            return cached
         scores = scores.to(torch.float16).contiguous()
         need = native.crf_decode_workspace_bytes(n, t, state_len)
-        import threading
         key = (scores.device, threading.get_ident(), slot)
         ws = self._ws_by_device.get(key)
         if ws is None or ws.numel() < need:

@@ -41,7 +41,7 @@ def shapes():
     # hac: 512 chunks x 9996 samples, stride 6 -> T = 1666 frames; tiles of TB = 64 chunks, 8-CTA clusters (CW = 192)
     N, T, TB, CS, H = 512, 1666, 64, 8, 384
     nt = N // TB
-    Tp = -(-max(9 + 9996, (T - 1) * 6 + 19) // 6)       # padded frames of the stem output (engine._tile_buffers)
+    Tp = -(-max(9 + 9996, (T - 1) * 6 + 19) // 6)       # padded frames of the stem output (LstmCrfPlan._buffers)
     CW = 4 * H // CS
     out = [
         ("hac_conv", dict(m=N * Tp, n=H, k=19 * 16, lda=6 * 16, ldc=H, act="tanh", bias=True,
