@@ -204,26 +204,25 @@ def band_align(query, target, chain, W):
         d = dg + s
         fo = up_h - 6 >= up_f - 2
         fv = np.where(fo, up_h - 6, up_f - 2)
-        # E by the recurrence, cell by cell
-        e = np.full(B, NEG, np.int64)
-        eo = np.zeros(B, dtype=bool)
-        h = np.full(B, NEG, np.int64)
-        sr = np.zeros(B, dtype=np.uint8)
+        # E by the recurrence, cell by cell (on Python lists: the band is up to 8193 cells wide)
+        e, eo, h, sr = [NEG] * B, [False] * B, [NEG] * B, [0] * B
+        inb_l, j_l, d_l, fv_l = inb.tolist(), j.tolist(), d.tolist(), fv.tolist()
         for x in range(B):
-            if not inb[x]:
+            if not inb_l[x]:
                 continue
-            if j[x] == 1:
+            if j_l[x] == 1:
                 e[x], eo[x] = max(0 - 6, NEG - 2), True
-            elif x > 0 and inb[x - 1]:
+            elif x > 0 and inb_l[x - 1]:
                 eo[x] = h[x - 1] - 6 >= e[x - 1] - 2
                 e[x] = h[x - 1] - 6 if eo[x] else e[x - 1] - 2
-            m3 = max(d[x], e[x], fv[x])
+            m3 = max(d_l[x], e[x], fv_l[x])
             if m3 <= 0:
                 h[x], sr[x] = 0, 1
             else:
-                h[x], sr[x] = m3, (0 if m3 == d[x] else (3 if m3 == e[x] else 2))
-            if h[x] > 0 and (h[x], i, j[x]) > best:
-                best = (int(h[x]), i, int(j[x]))
+                h[x], sr[x] = m3, (0 if m3 == d_l[x] else (3 if m3 == e[x] else 2))
+            if h[x] > 0 and (h[x], i, j_l[x]) > best:
+                best = (h[x], i, j_l[x])
+        h = np.array(h, dtype=np.int64)
         src[i], eob[i], fob[i] = sr, eo, fo
         hp, fp = h, np.where(inb, fv, NEG)
         lo_prev = lo

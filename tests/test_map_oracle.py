@@ -183,6 +183,23 @@ def test_band_align_equals_full_matrix(seed):
         assert got == want, (seed, W)
 
 
+@pytest.mark.parametrize("W", [0, 1, 5, 16])
+def test_band_align_equals_full_matrix_at_band_edges(W):
+    """First rows whose band starts at column 0, 1 or 2, a steep chain segment (the centre jumps by more than 2W + 1), a
+    flat one, and query overhangs that leave whole rows outside the target."""
+    rng = random.Random(100 + W)
+    t = _rand(rng, 60)
+    cases = [(t[:40], t[:50], [(0, 0), (39, 39)]), (t[W:W + 30], t, [(0, W), (29, W + 29)]),
+             (t[W + 1:W + 31], t, [(0, W + 1), (29, W + 30)]),
+             (t[:15] + t[45:60], t, [(0, 0), (14, 14), (15, 45), (29, 59)]),
+             (t[:10] + _rand(rng, 20) + t[10:25], t[:25], [(0, 0), (9, 9), (30, 10), (44, 24)]),
+             (_rand(rng, 12) + t[:30] + _rand(rng, 12), t[:30], [(12, 0), (41, 29)])]
+    for q, tt, chain in cases:
+        cen = O.centres(chain, len(q))
+        want = _brute_local(q, tt, lambda i, j: 0 <= j - (cen[i - 1] + 1 - W) <= 2 * W)
+        assert O.band_align(q, tt, chain, W) == want, (W, chain)
+
+
 def test_band_align_zero_score():
     assert O.band_align(b"AAAA", b"CCCC", [(0, 0), (3, 3)], 4) == (0, 0, 0, 0, 0, b"")
 
