@@ -334,7 +334,9 @@ int b200_stream_create(void** stream_out) {
 }
 
 int b200_quantize_i8(const void* x, void* out, long long n, float scale, void* stream) {
-    B200_REQUIRE(x && out && n >= 0, "quantize_i8: bad arguments");
+    B200_REQUIRE(n >= 0, "quantize_i8: bad element count %lld", n);
+    if (n == 0) return 0;   // an empty tensor may have a null data pointer
+    B200_REQUIRE(x && out, "quantize_i8: null pointer argument");
     return launch_quantize_i8((const __half*)x, (int8_t*)out, n, scale, (cudaStream_t)stream);
 }
 

@@ -233,6 +233,7 @@ conv_stem_tc_kernel(const __half* __restrict__ x, int L, const __half* __restric
 int launch_conv_stem(const __half* x, int N, int L, int C1, int K1, const __half* w1, const __half* b1, int act1,
                      int C2, int K2, const __half* w2, const __half* b2, int act2, __half* out, int Lp, int padl,
                      float lo1, float hi1, float lo2, float hi2, cudaStream_t stream) {
+    B200_REQUIRE(N <= 65535, "conv_stem: at most 65535 chunks per call (n=%d): the chunk index is gridDim.y", N);
     dim3 grid((Lp + TL - 1) / TL, N);
     const char* impl = getenv("B200_STEM_IMPL");   // "fma": the CUDA-core kernel for every shape
     if (C1 == 16 && K1 == 5 && C2 == 16 && K2 == 5 && !(impl && impl[0] == 'f')) {

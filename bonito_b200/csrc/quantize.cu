@@ -57,6 +57,7 @@ int launch_chunk_signal(const void* signal, int is_f32, long long length, int ch
     B200_REQUIRE(length > 0 && chunksize > 0 && overlap >= 0 && overlap < chunksize && row_stride >= chunksize,
                  "chunk_signal: bad geometry (length %lld, chunksize %d, overlap %d)", length, chunksize, overlap);
     const int n = chunk_count(length, chunksize, overlap), step = chunksize - overlap;
+    B200_REQUIRE(n <= 65535, "chunk_signal: at most 65535 chunks per read (%d): the chunk index is gridDim.y", n);
     const int stub = length < chunksize ? 0 : (int)((length - overlap) % step);
     const dim3 grid((unsigned)((chunksize + 255) / 256), (unsigned)n);
     if (is_f32) chunk_kernel<float><<<grid, 256, 0, stream>>>((const float*)signal, length, chunksize, step, stub, out, row_stride);

@@ -356,6 +356,7 @@ attention_kernel(const __half* __restrict__ qkv, const __half* __restrict__ cs, 
 int launch_conv_first(const __half* x, int N, int L, int C, int K, const __half* w, const __half* bias, int act,
                       __half* out, int Lp, int padl, cudaStream_t stream) {
     B200_REQUIRE(C % 8 == 0 && C <= 128 && K % 2 == 1 && K <= 15, "conv_first: unsupported shape 1->%d (k%d)", C, K);
+    B200_REQUIRE(N <= 65535, "conv_first: at most 65535 chunks per call (n=%d): the chunk index is gridDim.y", N);
     dim3 grid((Lp + CF_THREADS - 1) / CF_THREADS, N);
     const size_t smem = (size_t)(K * C + C + CF_THREADS + K) * sizeof(float);
     conv_first_kernel<<<grid, CF_THREADS, smem, stream>>>(x, L, w, bias, C, K, act, out, Lp, padl);

@@ -1,6 +1,8 @@
 """
-Shared pieces of the edge tests (test_gpu_kernel_edges.py, test_gpu_attention_edges.py, test_gpu_lstm_wide_edges.py):
-canary-filled output buffers, the fp16 interval checks and the float64 LSTM recurrence with its carried error bound.
+Shared pieces of the edge tests (test_gpu_kernel_edges.py, test_gpu_attention_edges.py, test_gpu_lstm_wide_edges.py,
+test_gpu_stem_edges.py):
+canary-filled output buffers, the fp16 interval checks, the interval of every epilogue activation, the GEMM epilogue's
+output map and the float64 LSTM recurrence with its carried error bound.
 
 Every output buffer is allocated with margins around the region a call may write and filled with a canary bit pattern
 (fp16: the NaN 0x7E5A, which no kernel produces; bytes: 0xA5).  After the call, every element the documented map addresses
@@ -64,6 +66,77 @@ def pre16(v, g):
 
 def _sigmoid(x):
     return 0.5 * (1.0 + np.tanh(0.5 * x))
+
+
+def _swish(x):
+    return x * _sigmoid(x)
+
+
+SWISH_ARGMIN = -1.278464542761074            # swish's only stationary point: 1 + x (1 - sigmoid(x)) = 0
+
+
+def act_interval(p_lo, p_hi, act, lo, hi):
+    """Interval of apply_act_f16's result when its fp16-rounded input is any fp16 value in [p_lo, p_hi].  Every activation
+    but swish is monotone, so its ends are those of the end points; swish falls to its minimum at SWISH_ARGMIN, which is
+    taken in wherever the interval straddles it."""
+    p_lo, p_hi = np.asarray(p_lo, dtype=np.float64), np.asarray(p_hi, dtype=np.float64)
+    out_lo, out_hi = None, None
+    for p in (p_lo, p_hi):
+        if act == 0:                                 # NONE
+            a, b = p, p
+        elif act in (1, 7):                          # SWISH, SWISH_CLAMP
+            s = _swish(p)
+            a, b = rn16(s - E_SFU * (1 + np.abs(p))), rn16(s + E_SFU * (1 + np.abs(p)))
+        elif act == 2:                               # TANH
+            t = np.tanh(p)
+            a, b = rn16(t - E_SFU), rn16(t + E_SFU)
+        elif act == 3:                               # CLAMP
+            a = b = np.clip(p, lo, hi)
+        elif act == 4:                               # SCALE: one fp32 multiply, then fp16
+            s = p * np.float32(lo)
+            a, b = rn16(s - 2.0 ** -24 * np.abs(s)), rn16(s + 2.0 ** -24 * np.abs(s))
+        elif act == 6:                               # TANH_SCALE: fp16(fp16(tanh) * lo)
+            t = np.tanh(p)
+            m_lo, m_hi = rn16(t - E_SFU), rn16(t + E_SFU)
+            s1, s2 = m_lo * np.float32(lo), m_hi * np.float32(lo)
+            s_lo, s_hi = np.minimum(s1, s2), np.maximum(s1, s2)
+            a, b = rn16(s_lo - 2.0 ** -24 * np.abs(s_lo)), rn16(s_hi + 2.0 ** -24 * np.abs(s_hi))
+        elif act == 8:                               # RELU
+            a = b = np.maximum(p, 0.0)
+        else:
+            raise ValueError(act)
+        out_lo = a if out_lo is None else np.minimum(out_lo, a)
+        out_hi = b if out_hi is None else np.maximum(out_hi, b)
+    if act in (1, 7):
+        s_min = rn16(_swish(SWISH_ARGMIN) - E_SFU * (1 - SWISH_ARGMIN))
+        out_lo = np.where((p_lo < SWISH_ARGMIN) & (p_hi > SWISH_ARGMIN), np.minimum(out_lo, s_min), out_lo)
+        if act == 7:
+            out_lo, out_hi = np.clip(out_lo, lo, hi), np.clip(out_hi, lo, hi)
+    return out_lo, out_hi
+
+
+def gemm_rows(m, rows_inner, valid_inner, stride_inner, stride_outer, group, stride_group):
+    """Output row of every input row under the GEMM epilogue's row map (b200_gemm_fwd_ex), -1 for dropped rows."""
+    r = np.arange(m)
+    outer, inner = r // rows_inner, r % rows_inner
+    if group > 0:
+        row = inner * stride_inner + (outer % group) * stride_outer + (outer // group) * stride_group
+    else:
+        row = inner * stride_inner + outer * stride_outer
+    return np.where(inner < valid_inner, row, -1)
+
+
+def gemm_dest(m, n, rows_inner, valid_inner, stride_inner, stride_outer, group, stride_group, cb_width, cb_rows, ldc):
+    """Flat output index (relative to c) of every (input row, column) the documented map writes, -1 for dropped rows."""
+    row = gemm_rows(m, rows_inner, valid_inner, stride_inner, stride_outer, group, stride_group)
+    col = np.arange(n)
+    if cb_width > 0:
+        rows = row[:, None] + (col // cb_width)[None, :] * cb_rows
+        cols = np.broadcast_to(col % cb_width, (m, n))
+    else:
+        rows, cols = np.broadcast_to(row[:, None], (m, n)), np.broadcast_to(col, (m, n))
+    dest = rows * ldc + cols
+    return np.where((row >= 0)[:, None], dest, -1)
 
 
 # ------------------------------------------------------------------------------------------------ LSTM recurrences

@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_kernel_edges import CANARY16, E_SFU, _swish, act_interval, pre16, rn16
+from _edges import CANARY16, E_SFU, _swish, act_interval, pre16, rn16
 
 pytestmark = pytest.mark.gpu
 

@@ -19,8 +19,8 @@ import numpy as np
 import pytest
 import torch
 
-from _edges import (CANARY8, CANARY16, CANARY32, E_SFU, _lstm_inputs, _lstm_reference, _perm_hh, _sigmoid, bits16,
-                    canary16, check_between, check_guarded, pre16, rn16)
+from _edges import (CANARY8, CANARY16, CANARY32, E_SFU, _lstm_inputs, _lstm_reference, _perm_hh, _swish, act_interval,
+                    bits16, canary16, check_between, check_guarded, gemm_dest, pre16, rn16)
 from oracle import crf_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -34,62 +34,6 @@ def native():
     from bonito_b200 import native as nat
     nat.require()
     return nat
-
-
-def _swish(x):
-    return x * _sigmoid(x)
-
-
-def act_interval(p_lo, p_hi, act, lo, hi):
-    """Interval of apply_act_f16's result when its fp16-rounded input is p_lo or p_hi (consecutive fp16 values)."""
-    out_lo, out_hi = None, None
-    for p in (p_lo, p_hi):
-        if act == 0:                                 # NONE
-            a, b = p, p
-        elif act in (1, 7):                          # SWISH, SWISH_CLAMP
-            s = _swish(p)
-            a, b = rn16(s - E_SFU * (1 + np.abs(p))), rn16(s + E_SFU * (1 + np.abs(p)))
-            if act == 7:
-                a, b = np.clip(a, lo, hi), np.clip(b, lo, hi)
-        elif act == 2:                               # TANH
-            t = np.tanh(p)
-            a, b = rn16(t - E_SFU), rn16(t + E_SFU)
-        elif act == 3:                               # CLAMP
-            a = b = np.clip(p, lo, hi)
-        elif act == 4:                               # SCALE: one fp32 multiply, then fp16
-            s = p * np.float32(lo)
-            a, b = rn16(s - 2.0 ** -24 * np.abs(s)), rn16(s + 2.0 ** -24 * np.abs(s))
-        elif act == 6:                               # TANH_SCALE: fp16(fp16(tanh) * lo)
-            t = np.tanh(p)
-            m_lo, m_hi = rn16(t - E_SFU), rn16(t + E_SFU)
-            s1, s2 = m_lo * np.float32(lo), m_hi * np.float32(lo)
-            s_lo, s_hi = np.minimum(s1, s2), np.maximum(s1, s2)
-            a, b = rn16(s_lo - 2.0 ** -24 * np.abs(s_lo)), rn16(s_hi + 2.0 ** -24 * np.abs(s_hi))
-        elif act == 8:                               # RELU
-            a = b = np.maximum(p, 0.0)
-        else:
-            raise ValueError(act)
-        out_lo = a if out_lo is None else np.minimum(out_lo, a)
-        out_hi = b if out_hi is None else np.maximum(out_hi, b)
-    return out_lo, out_hi
-
-
-def gemm_dest(m, n, rows_inner, valid_inner, stride_inner, stride_outer, group, stride_group, cb_width, cb_rows, ldc):
-    """Flat output index (relative to c) of every (input row, column) the documented map writes, -1 for dropped rows."""
-    r = np.arange(m)
-    outer, inner = r // rows_inner, r % rows_inner
-    if group > 0:
-        row = inner * stride_inner + (outer % group) * stride_outer + (outer // group) * stride_group
-    else:
-        row = inner * stride_inner + outer * stride_outer
-    col = np.arange(n)
-    if cb_width > 0:
-        rows = row[:, None] + (col // cb_width)[None, :] * cb_rows
-        cols = np.broadcast_to(col % cb_width, (m, n))
-    else:
-        rows, cols = np.broadcast_to(row[:, None], (m, n)), np.broadcast_to(col, (m, n))
-    dest = rows * ldc + cols
-    return np.where((inner < valid_inner)[:, None], dest, -1)
 
 
 # ------------------------------------------------------------------------------------------------ fp16 GEMMs
