@@ -39,6 +39,8 @@ int lstm_rec_tile_cluster(int hidden);
 int launch_lstm_rec_tile(const __half* gx, const __half* whh, __half* y, void* workspace, int T, int N, int hidden,
                          int reverse, cudaStream_t stream);
 size_t lstm_rec_tile_workspace_bytes(int N);
+int launch_lstm_fused_tile(const __half* x, const __half* wih, const __half* bias, const __half* whh, __half* y,
+                           void* workspace, int T, int N, int hidden, int reverse, cudaStream_t stream);
 int lstm_rec_wide_ctas(int hidden);
 size_t lstm_rec_wide_workspace_bytes(int N, int hidden);
 size_t lstm_rec_wide_status_offset(int N, int hidden);
@@ -270,6 +272,15 @@ int b200_lstm_rec_tile_fwd(const void* gx, const void* whh, void* y, void* works
     if (t == 0 || n == 0) return 0;
     return launch_lstm_rec_tile((const __half*)gx, (const __half*)whh, (__half*)y, workspace, t, n, hidden, reverse,
                                (cudaStream_t)stream);
+}
+
+int b200_lstm_fused_tile_fwd(const void* x, const void* wih, const void* bias, const void* whh, void* y, void* workspace,
+                             int t, int n, int hidden, int reverse, void* stream) {
+    B200_REQUIRE(x && wih && bias && whh && y && workspace, "lstm_fused_tile: null pointer argument");
+    B200_REQUIRE(t >= 0 && n >= 0, "lstm_fused_tile: bad sizes t=%d n=%d", t, n);
+    if (t == 0 || n == 0) return 0;
+    return launch_lstm_fused_tile((const __half*)x, (const __half*)wih, (const __half*)bias, (const __half*)whh, (__half*)y,
+                                  workspace, t, n, hidden, reverse, (cudaStream_t)stream);
 }
 
 int b200_lstm_wide_ctas(int hidden) { return lstm_rec_wide_ctas(hidden); }

@@ -22,11 +22,13 @@ more GEMM; these layers and learned blank scores run on the wide layout (H = 768
 Every layout shares the front end: the fused conv1 + conv2 stem writes `[N][Lp][C2]` channels last, and the strided conv3 is
 one GEMM over the overlapping-row view of it.  The LSTM width picks one of three activation layouts (`LstmCrfPlan.forward`):
 
-* Tile layout, width 384 (hac, the headline path; `forward_tiles`): activations tile-major `[tile][T][64][H]`, gate
-  pre-activations `[tile][T][8][64][192]`; layer by layer on the current stream, per layer ONE input GEMM over all tiles
-  and ONE launch of the wgmma recurrent kernel (one 8-CTA cluster per 64-chunk tile, 8 clusters for 512 chunks).  The
-  whole encoder is one C call (`b200_lstm_crf_fwd`) unless per-kernel events, intermediate activations, another GEMM
-  implementation or the int8 input projection ask for the launches one at a time.  Buffers are cached per (batch, chunk
+* Tile layout, width 384 (hac, the headline path; `forward_tiles`): activations tile-major `[tile][T][64][H]`; layer by
+  layer on the current stream, per layer ONE launch of the fused wgmma LSTM kernel (lstm_fused_tile.cu: one 8-CTA cluster
+  per 64-chunk tile, 8 clusters for 512 chunks), which computes the input projection inside the recurrence.  Under
+  `--quantize` the input projection is an int8 GEMM into gate pre-activations `[tile][T][8][64][192]` instead, followed by
+  the unfused recurrent kernel (lstm_rec_tile.cu).  The whole encoder is one C call (`b200_lstm_crf_fwd`) unless per-kernel
+  events, intermediate activations, another GEMM implementation or the int8 input projection ask for the launches one at
+  a time.  Buffers are cached per (batch, chunk
   length, slot): `slot` selects one of several independent buffer sets, so that consecutive batches can be in flight on
   different streams (`score_batches`, bench.py).
 
@@ -311,7 +313,8 @@ class LstmCrfPlan:
                 # zero-filled once: rows of chunks beyond the batch (last tile) are never written and must stay finite
                 ya=torch.zeros(nt, T, TB, H, dtype=f16, device=dev),
                 yb=torch.zeros(nt, T, TB, H, dtype=f16, device=dev),
-                gx=torch.zeros(nt, T, CS, TB, 4 * H // CS, dtype=f16, device=dev),
+                # gate pre-activations of the int8 input projection; the fp16 layers compute them inside the recurrence
+                gx=torch.zeros(nt, T, CS, TB, 4 * H // CS, dtype=f16, device=dev) if self.quantize else None,
                 yq=torch.empty(nt * T * TB * H, dtype=torch.int8, device=dev) if self.quantize else None,
                 # staging of the recurrent kernel's h all-gather: one region per tile (the clusters run concurrently)
                 hx=torch.empty(nt, native.lstm_rec_tile_workspace_bytes(TB), dtype=torch.uint8, device=dev),
@@ -441,8 +444,8 @@ class LstmCrfPlan:
 
     def forward_tiles(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, return_features=False, slot=0):
         """
-        Forward in the tile layout, layer by layer on the current stream: one input-projection GEMM and ONE recurrent launch
-        (a cluster per tile, all in one wave) per layer.  `slot` selects one of several independent buffer sets (batches in
+        Forward in the tile layout, layer by layer on the current stream: ONE launch of the fused LSTM kernel (a cluster per
+        tile, all in one wave) per layer, or the int8 input-projection GEMM and the recurrent kernel under `quantize`.  `slot` selects one of several independent buffer sets (batches in
         flight at the same time).
         """
         x = self._input(x)
@@ -472,19 +475,19 @@ class LstmCrfPlan:
             feats["conv"] = gather(cur)
         rows = dict(rows_inner=TB, valid_inner=TB, stride_inner=1, stride_outer=CS * TB, cb_width=CW, cb_rows=TB)
         for li, layer in enumerate(self.lstm):
-            # rows (tile, t, chunk) -> gx[tile][t][rank][chunk][CW]
             if self.quantize:
+                # rows (tile, t, chunk) -> gx[tile][t][rank][chunk][CW]
                 with _Stage("quantize_i8", events):
                     native.quantize_i8(cur, b["yq"], 127.0)
                 with _Stage("lstm_in_gemm", events):
                     native.gemm_i8(b["yq"], H, layer["wih_q"], layer["wih_scale"], layer["bias"], b["gx"], CW, nt * T * TB,
                                    4 * H, H, **rows)
+                with _Stage("lstm_rec", events):
+                    native.lstm_rec_tile(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"], workspace=b["hx"])
             else:
-                with _Stage("lstm_in_gemm", events):
-                    native.gemm(cur, H, layer["wih"], layer["bias"], b["gx"], CW, nt * T * TB, 4 * H, H, impl=gemm_impl,
-                                **rows)
-            with _Stage("lstm_rec", events):
-                native.lstm_rec_tile(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"], workspace=b["hx"])
+                with _Stage("lstm_rec", events):
+                    native.lstm_fused_tile(cur, layer["wih"], layer["bias"], layer["whh"], nxt, T, N, H, layer["reverse"],
+                                           workspace=b["hx"])
             cur, nxt = nxt, cur
             if feats is not None:
                 feats[f"lstm{li}"] = gather(cur)

@@ -73,6 +73,8 @@ SIGNATURES = {
     "b200_lstm_tile_cluster": (c_int, [c_int]),
     "b200_lstm_rec_tile_workspace_bytes": (c_size_t, [c_int]),
     "b200_lstm_rec_tile_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "b200_lstm_fused_tile_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                         c_int, c_void_p]),
     "b200_lstm_wide_ctas": (c_int, [c_int]),
     "b200_lstm_wide_max_chunks": (c_int, [c_int]),
     "b200_lstm_wide_resident": (c_int, [c_int]),
@@ -405,6 +407,20 @@ def lstm_rec_tile(gx, whh, y, t, n, hidden, reverse, stream=None, workspace=None
         rc = lib.b200_lstm_rec_tile_fwd(_ptr(gx), _ptr(_f16(whh, "whh")), _ptr(y), _ptr(workspace), t, n, hidden,
                                         int(bool(reverse)), _stream(stream))
     _check(rc, "b200_lstm_rec_tile_fwd")
+    return y
+
+
+def lstm_fused_tile(x, wih, bias, whh, y, t, n, hidden, reverse, stream=None, workspace=None):
+    """One whole fp16 LSTM layer in the tile layout, input projection included: x, y [tiles][T][64][H]; wih / bias in gx
+    column order, whh in W_hh row order (see b200_lstm_fused_tile_fwd).  `workspace`: uint8 tensor of
+    lstm_rec_tile_workspace_bytes(n) bytes (allocated here when omitted)."""
+    lib = require()
+    if workspace is None:
+        workspace = torch.empty(lstm_rec_tile_workspace_bytes(n), dtype=torch.uint8, device=y.device)
+    with torch.cuda.device(y.device):
+        rc = lib.b200_lstm_fused_tile_fwd(_ptr(x), _ptr(_f16(wih, "wih")), _ptr(_f16(bias, "bias")), _ptr(_f16(whh, "whh")),
+                                          _ptr(y), _ptr(workspace), t, n, hidden, int(bool(reverse)), _stream(stream))
+    _check(rc, "b200_lstm_fused_tile_fwd")
     return y
 
 

@@ -147,6 +147,19 @@ int b200_lstm_rec_tile_fwd(const void* gx, const void* whh, void* y, void* works
                            int reverse, void* stream);
 
 /*
+ * One whole fp16 LSTM layer of hidden = 384 in the tile layout, input projection included (the hot path of the hac model):
+ * the same clusters, tiles and h all-gather as b200_lstm_rec_tile_fwd, with x_t W_ih^T + b computed inside the recurrence
+ * (W_ih slice resident in shared memory, x_t loaded by TMA), so no gate pre-activations go through HBM.  The results are
+ * bit-identical to b200_gemm_fwd_ex (wih, bias) into gx followed by b200_lstm_rec_tile_fwd.
+ *   x    [tiles][T][64][H]  layer input (rows of chunks >= n are read and their results dropped: keep them finite)
+ *   wih  [4H][H], bias [4H] rows in gx column order [unit][gate i,f,g,o];  whh [4H][H] as for b200_lstm_rec_fwd
+ *   y    [tiles][T][64][H]  h_t in natural unit order; rows of chunks >= n are not written
+ *   workspace               b200_lstm_rec_tile_workspace_bytes(n) bytes, as for b200_lstm_rec_tile_fwd
+ */
+int b200_lstm_fused_tile_fwd(const void* x, const void* wih, const void* bias, const void* whh, void* y, void* workspace,
+                             int t, int n, int hidden, int reverse, void* stream);
+
+/*
  * Wide recurrent kernel, hidden = 768 and 1024 (dna_r9.4.1@v3.1, dna_r10.4.1@v4.3): W_hh is spread over G = hidden / 8 CTAs
  * (8 units = 32 gate columns each, slice resident in shared memory), one cooperative launch per layer, wgmma on 64-chunk
  * tiles, h exchanged through L2 with a grid-wide barrier every step.  b200_lstm_cluster_size() keeps returning 0 for these
@@ -327,16 +340,16 @@ int b200_gemm_i8_fwd(const void* a, long long lda, const void* b, const void* co
 
 /*
  * ---- coarse entry point: the whole LSTM-CRF encoder forward of one batch from one call ----
- * conv stem -> strided convolution (GEMM) -> n_lstm x (input projection GEMM + persistent recurrent layer) ->
- * LinearCRFEncoder GEMM (+Clamp), enqueued on `stream` (14 launches for the hac shape).  Replaces the module-tree walk of
+ * conv stem -> strided convolution (GEMM) -> n_lstm x fused LSTM layer (b200_lstm_fused_tile_fwd) -> LinearCRFEncoder
+ * GEMM (+Clamp), enqueued on `stream` (9 launches for the hac shape).  Replaces the module-tree walk of
  * `Serial.forward` over the encoder of a bonito.crf model (bonito/nn.py:82-89, bonito/crf/model.py:150-162) -- the span
  * `Model.use_koi` swaps for koi.lstm.update_graph plus the layers around it.  Tile-layout recurrent kernel only
  * (b200_lstm_tile_chunks(hidden) > 0).  The plan holds DEVICE pointers to packed weights (layouts as documented for the
  * fine-grained entry points above: conv weights in torch layout, w3 [H][k3*c2] with k = tap*c2 + cin, wih / bias in gx column
  * order, whh in W_hh row order) and to caller-owned work buffers:
- *   stem  (n*tp*s3*c2 + k3*c2) halves, the last k3*c2 zeroed       ya, yb  tiles*t*48*H halves, zero-filled once
- *   gx    tiles*t*4H*48 halves, zero-filled once                    hx      b200_lstm_rec_tile_workspace_bytes(n) bytes
- * with tiles = ceil(n / 48), t = frames, tp = padded frames per chunk (the stem buffer holds tp*s3 samples per chunk).
+ *   stem  (n*tp*s3*c2 + k3*c2) halves, the last k3*c2 zeroed       ya, yb  tiles*t*64*H halves, zero-filled once
+ *   gx    unused (may be NULL)                                      hx      b200_lstm_rec_tile_workspace_bytes(n) bytes
+ * with tiles = ceil(n / 64), t = frames, tp = padded frames per chunk (the stem buffer holds tp*s3 samples per chunk).
  * x [n][l] fp16 -> scores [n][t][n_scores] fp16 (no blank column).
  */
 #define B200_MAX_LSTM_LAYERS 8
