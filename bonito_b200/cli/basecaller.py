@@ -1,9 +1,10 @@
 """
 `bonito_b200 basecaller <model_directory> <reads_directory>` -- the flag surface of the reference's
 `bonito basecaller` (`bonito/cli/basecaller.py:168-199`) over the native engine.
-Output is FASTQ, or SAM text with the `mv:B:c` move table when stdout is redirected to a `.sam` file (the reference's
-`biofmt` rule, bonito/io.py:35-54).  `--reference <fasta>` maps the calls on the GPU (bonito_b200.aligner, this
-project's rules in place of minimap2's) and writes aligned SAM; `--alignment-threads` is accepted and has no effect.  CTC
+Output is FASTQ, or SAM text with the `mv:B:c` move table when stdout is redirected to a `.sam` file, or BAM with the same
+records when it is redirected to a `.bam` file, BGZF-compressed on the GPU (the reference's `biofmt` rule,
+bonito/io.py:35-54); CRAM is refused.  `--reference <fasta>` maps the calls on the GPU (bonito_b200.aligner, this
+project's rules in place of minimap2's) and writes aligned SAM or BAM; `--alignment-threads` is accepted and has no effect.  CTC
 training-data export (`--save-ctc`) exits with an explanation.
 `B200_CTC_BEAMSIZE=W` in the environment (1..32, unset = 1, the greedy decode) decodes the QuartzNet CTC models with the
 prefix beam search of width W; the flag surface itself is the reference's and has no beam option.
@@ -20,7 +21,7 @@ import numpy as np
 
 from bonito_b200.aligner import PRESETS, Aligner, IndexBuildError, align_map
 from bonito_b200.ctc.model import MAX_BEAMSIZE, Model as CtcModel
-from bonito_b200.io import Writer, biofmt
+from bonito_b200.io import BamWriter, Writer, biofmt
 from bonito_b200.nn import fuse_bn_
 from bonito_b200.reader import Reader
 from bonito_b200.util import init, load_model, load_symbol
@@ -48,8 +49,9 @@ def main(args):
         sys.stderr.write("> error: no suitable files found in %s\n" % args.reads_directory)
         exit(1)
     fmt = biofmt(aligned=args.reference is not None)
-    if fmt.mode not in ("wfq", "w"):
-        sys.stderr.write(f"> error: {fmt.name} output needs htslib, which this build does not bundle; redirect to .sam or .fastq\n")
+    if fmt.mode not in ("wfq", "w", "wb"):
+        sys.stderr.write(f"> error: {fmt.name} output needs htslib, which this build does not bundle; "
+                         "redirect to .bam, .sam or .fastq\n")
         exit(1)
     if args.reference and fmt.name == "fastq":
         sys.stderr.write(f"> warning: did you really want {fmt.aligned} {fmt.name}?\n")
@@ -109,9 +111,12 @@ def main(args):
                        chunksize=params["chunksize"], overlap=params["overlap"], **decode_args)
     if aligner:
         results = align_map(aligner, results, n_thread=args.alignment_threads)
-    writer = Writer(results, min_qscore=args.min_qscore, mode=fmt.mode,
-                    group_key=os.path.basename(os.path.normpath(args.model_directory)),
-                    contigs=aligner.contigs if aligner else None)
+    writer_args = dict(min_qscore=args.min_qscore, group_key=os.path.basename(os.path.normpath(args.model_directory)),
+                       contigs=aligner.contigs if aligner else None)
+    if fmt.mode == "wb":
+        writer = BamWriter(results, device=args.device, **writer_args)
+    else:
+        writer = Writer(results, mode=fmt.mode, **writer_args)
     t0 = perf_counter()
     writer.start()
     writer.join()

@@ -4,6 +4,8 @@ flag surface and the printed summary of the reference's `bonito duplex` (bonito/
 bonito_b200/duplex.py; the alignments of a batch of pairs run as GPU launches (b200_pair_align) on a background thread
 while a pool of `--threads` host threads builds the consensus of the previous batch.
 
+Output: FASTQ, SAM text or BAM (BGZF-compressed on the GPU), chosen by the extension stdout is redirected to; CRAM is
+refused.
 Input: SAM text (`.sam`, what `basecaller` writes when redirected to a .sam file) or FASTQ (`.fastq` / `.fq`), chosen by
 the extension.  For each read id the first record that is neither secondary (0x100) nor supplementary (0x800) is used,
 SEQ and QUAL as stored (reverse-strand records included, as pysam's query_sequence gives them).  BAM / CRAM input and
@@ -21,7 +23,7 @@ from time import perf_counter
 import numpy as np
 
 from bonito_b200 import duplex, native
-from bonito_b200.io import DuplexWriter, biofmt
+from bonito_b200.io import DuplexBamWriter, DuplexWriter, biofmt
 from bonito_b200.multiprocessing import thread_iter
 
 BATCH_PAIRS = 1024               # pairs per GPU batch
@@ -154,8 +156,8 @@ def main(args):
     except ValueError as err:
         _fail(str(err))
     fmt = biofmt(aligned=False)
-    if fmt.mode not in ("wfq", "w"):
-        _fail(f"{fmt.name} output needs htslib, which this build does not bundle; redirect to .sam or .fastq")
+    if fmt.mode not in ("wfq", "w", "wb"):
+        _fail(f"{fmt.name} output needs htslib, which this build does not bundle; redirect to .bam, .sam or .fastq")
     sys.stderr.write(f"> outputting {fmt.aligned} {fmt.name}\n")
 
     pairs = read_pairs(args.duplex_pairs_file, header=not args.no_header)
@@ -168,7 +170,11 @@ def main(args):
     counts = {}
     t0 = perf_counter()
     with ThreadPoolExecutor(max(1, args.threads)) as pool:
-        writer = DuplexWriter(call(pairs, reads, pool, counts=counts), mode=fmt.mode, min_qscore=args.min_qscore)
+        results = call(pairs, reads, pool, counts=counts)
+        if fmt.mode == "wb":
+            writer = DuplexBamWriter(results, min_qscore=args.min_qscore)
+        else:
+            writer = DuplexWriter(results, mode=fmt.mode, min_qscore=args.min_qscore)
         writer.start()
         writer.join()
     duration = perf_counter() - t0

@@ -1,9 +1,10 @@
 """
-pysam-free output for `bonito_b200 basecaller`: FASTQ and SAM text (unaligned, or aligned by bonito_b200.aligner) with the
-reference's header, record and tag layout (`bonito/io.py:41-166,400-469`, `documentation/SAM.md`), including the
-sequence-to-signal move table `mv:B:c,<stride>,<moves...>` (`io.py:57-70,455-456`).  The reference writes through
-pysam / htslib; BAM / CRAM need htslib, which this build does not bundle, so those formats are refused with an
-explanation instead of being approximated.
+pysam-free output for `bonito_b200 basecaller` and `duplex`: FASTQ, SAM text (unaligned, or aligned by
+bonito_b200.aligner) and BAM, with the reference's header, record and tag layout (`bonito/io.py:41-166,400-469`,
+`documentation/SAM.md`), including the sequence-to-signal move table `mv:B:c,<stride>,<moves...>` (`io.py:57-70,455-456`).
+The reference writes through pysam / htslib.  Here BAM records are the binary encoding of the SAM lines this module
+builds (bonito_b200.bam), BGZF-compressed on the GPU; CRAM needs htslib, which this build does not bundle, so it is refused
+with an explanation instead of being approximated.
 Deviation: on the reverse strand QUAL is reversed along with SEQ, as the SAM specification requires; the reference
 reverse-complements SEQ and leaves QUAL as called.
 """
@@ -17,6 +18,7 @@ from threading import Thread
 import numpy as np
 
 from bonito_b200.aligner import revcomp
+from bonito_b200.bam import BamOutput
 from bonito_b200.util import mean_qscore_from_qstring
 
 __ont_bam_spec__ = "0.0.2"
@@ -134,8 +136,7 @@ class DuplexWriter(Thread):
 
     def run(self):
         try:
-            if self.mode == "w":
-                self.fd.write(sam_header())
+            self.begin()
             for (temp_id, comp_id), res in self.iterator:
                 read_id = f"{temp_id};{comp_id}"
                 seq, qstring = res["sequence"], res["qstring"]
@@ -143,14 +144,40 @@ class DuplexWriter(Thread):
                 self.log.append((read_id, len(seq)))
                 if mean_q < self.min_qscore or not len(seq):
                     continue
-                tags = [f"qs:i:{round(mean_q)}"]
-                if self.mode == "w":
-                    self.fd.write(sam_record(read_id, seq, qstring, tags=tags) + "\n")
-                else:
-                    write_fastq(read_id, seq, qstring, fd=self.fd, tags=tags)
-            self.fd.flush()
+                self.write_read(read_id, seq, qstring, [f"qs:i:{round(mean_q)}"])
+            self.end()
         except BaseException as err:   # surfaced by the CLI after join()
             self.error = err
+
+    def begin(self):
+        if self.mode == "w":
+            self.fd.write(sam_header())
+
+    def write_read(self, read_id, seq, qstring, tags):
+        if self.mode == "w":
+            self.fd.write(sam_record(read_id, seq, qstring, tags=tags) + "\n")
+        else:
+            write_fastq(read_id, seq, qstring, fd=self.fd, tags=tags)
+
+    def end(self):
+        self.fd.flush()
+
+
+class DuplexBamWriter(DuplexWriter):
+    """DuplexWriter to BAM: the records of its SAM mode, encoded by bonito_b200.bam onto the binary file `fd`."""
+
+    def __init__(self, iterator, fd=None, min_qscore=0, device="cuda", members_per_launch=256):
+        super().__init__(iterator, fd=fd if fd is not None else sys.stdout.buffer, min_qscore=min_qscore, mode="w")
+        self.device, self.members_per_launch = device, members_per_launch
+
+    def begin(self):
+        self.bam = BamOutput(self.fd, sam_header(), device=self.device, members_per_launch=self.members_per_launch)
+
+    def write_read(self, read_id, seq, qstring, tags):
+        self.bam.write_sam(sam_record(read_id, seq, qstring, tags=tags))
+
+    def end(self):
+        self.bam.close()
 
 
 class Writer(Thread):
@@ -172,21 +199,51 @@ class Writer(Thread):
 
     def run(self):
         try:
-            if self.mode == "w":
-                self.fd.write(sam_header(self.groups, contigs=self.contigs))
+            self.begin()
             for read, res in self.iterator:
                 seq, qstring = res["sequence"], res["qstring"]
                 samples = len(read.signal) + getattr(read, "trimmed_samples", 0)
                 if len(seq) and mean_qscore_from_qstring(qstring) >= self.min_qscore:
-                    if self.mode == "w":
-                        self.fd.write(sam_record(read.read_id, seq, qstring, mapping=res.get("mapping"),
-                                                tags=read_tags(read, res, self.group_key)) + "\n")
-                    else:
-                        write_fastq(read.read_id, seq, qstring, fd=self.fd,
-                                    tags=read_tags(read, res, self.group_key, with_moves=False) if self.tags else None)
+                    self.write_read(read, res, seq, qstring)
                     self.log.append((read.read_id, samples))
                 else:
                     sys.stderr.write(f"> skipping empty / low quality sequence {read.read_id}\n")
-            self.fd.flush()
+            self.end()
         except BaseException as err:   # surfaced by the CLI after join()
             self.error = err
+
+    def begin(self):
+        if self.mode == "w":
+            self.fd.write(sam_header(self.groups, contigs=self.contigs))
+
+    def sam_line(self, read, res, seq, qstring):
+        return sam_record(read.read_id, seq, qstring, mapping=res.get("mapping"), tags=read_tags(read, res, self.group_key))
+
+    def write_read(self, read, res, seq, qstring):
+        if self.mode == "w":
+            self.fd.write(self.sam_line(read, res, seq, qstring) + "\n")
+        else:
+            write_fastq(read.read_id, seq, qstring, fd=self.fd,
+                        tags=read_tags(read, res, self.group_key, with_moves=False) if self.tags else None)
+
+    def end(self):
+        self.fd.flush()
+
+
+class BamWriter(Writer):
+    """Writer to BAM: the header and records of its SAM mode, encoded by bonito_b200.bam onto the binary file `fd` (the
+    BGZF compression runs on `device`)."""
+
+    def __init__(self, iterator, fd=None, device="cuda", members_per_launch=256, **kwargs):
+        super().__init__(iterator, fd=fd if fd is not None else sys.stdout.buffer, mode="w", **kwargs)
+        self.device, self.members_per_launch = device, members_per_launch
+
+    def begin(self):
+        self.bam = BamOutput(self.fd, sam_header(self.groups, contigs=self.contigs), self.contigs, device=self.device,
+                             members_per_launch=self.members_per_launch)
+
+    def write_read(self, read, res, seq, qstring):
+        self.bam.write_sam(self.sam_line(read, res, seq, qstring))
+
+    def end(self):
+        self.bam.close()

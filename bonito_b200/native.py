@@ -118,7 +118,12 @@ SIGNATURES = {
     "b200_map_align_trace_bytes": (c_size_t, [c_int, c_int]),
     "b200_map_align": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                c_void_p]),
+    "b200_bgzf_workspace_bytes": (c_size_t, [c_longlong]),
+    "b200_bgzf_compress": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
+
+BGZF_MEMBER_INPUT = 65280   # B200_BGZF_MEMBER_INPUT
+BGZF_MEMBER_MAX = 65536     # output bytes per member at most
 
 
 class NativeError(RuntimeError):
@@ -811,3 +816,31 @@ def map_align(query, target, chain, meta, max_band, cen, trace, ops, out, stream
     with torch.cuda.device(out.device):
         _check(lib.b200_map_align(_ptr(query), _ptr(target), _ptr(chain), _ptr(meta), n, int(max_band), _ptr(cen), _ptr(trace),
                                   _ptr(ops), _ptr(out), _stream(stream)), "b200_map_align")
+
+
+# ------------------------------------------------------------------------------------------------ BGZF (bgzf.cu)
+def bgzf_members(in_bytes):
+    return -(-int(in_bytes) // BGZF_MEMBER_INPUT)
+
+
+def bgzf_workspace_bytes(in_bytes):
+    return load().b200_bgzf_workspace_bytes(int(in_bytes))
+
+
+def bgzf_compress(inp, out, out_offsets, workspace, stream=None):
+    """BGZF members of the CUDA uint8 buffer `inp`, back to back into `out` (CUDA uint8, >= members * 65536 bytes);
+    out_offsets (CUDA int64 [members + 1]) receives their offsets and the total length (see b200_bgzf_compress)."""
+    lib = require()
+    what = "bgzf_compress"
+    _dev(inp, torch.uint8, "inp", what)
+    _dev(out, torch.uint8, "out", what)
+    _dev(workspace, torch.uint8, "workspace", what)
+    n = bgzf_members(inp.numel())
+    _dev(out_offsets, torch.int64, "out_offsets", what)
+    if out_offsets.numel() < n + 1 or out.numel() < n * BGZF_MEMBER_MAX:
+        raise NativeError(f"{what}: {n} members need {n + 1} offsets and {n * BGZF_MEMBER_MAX} output bytes")
+    with torch.cuda.device(inp.device):
+        rc = lib.b200_bgzf_compress(_ptr(inp), inp.numel(), _ptr(out), _ptr(out_offsets), _ptr(workspace), workspace.numel(),
+                                    _stream(stream))
+    _check(rc, "b200_bgzf_compress")
+    return out_offsets

@@ -21,6 +21,8 @@
  *   b200_ctc_crf_*            koi.ctc (logZ_cu_sparse, fwd/bwd_scores_  bonito/crf/model.py:30-143
  *                             cu_sparse, logZ_cu, viterbi_alignments)
  *   b200_ctc_beam_search      fast_ctc_decode.beam_search             bonito/ctc/model.py:39-46, ctc/basecall.py:43-61
+ *   b200_bgzf_compress        htslib bgzf_write, reached through      bonito/io.py:400-503
+ *                             pysam AlignmentFile(..., 'wb') (BAM output)
  *
  * Conventions (SURVEY.md section 8b): every function returns 0 on success and a negative value on
  * failure, with a message available from b200_last_error().  All pointers are raw DEVICE pointers
@@ -470,6 +472,21 @@ int b200_map_extract(const void* akey, const void* aq, const void* f, const void
 size_t b200_map_align_trace_bytes(int query_len, int band);
 int b200_map_align(const void* query, const void* target, const void* chain, const void* meta, int n_pairs, int max_band,
                    void* cen, void* trace, void* ops, void* out, void* stream);
+
+/*
+ * ---- BGZF compression for BAM output (SAM specification section 4.1; the DEFLATE parse and codes are this library's,
+ *      stated in bonito_b200/csrc/bgzf.cu) ----
+ * in: DEVICE bytes [in_bytes], cut into n = ceil(in_bytes / B200_BGZF_MEMBER_INPUT) members in order, each of
+ * B200_BGZF_MEMBER_INPUT bytes but the last (in_bytes == 0: no members).  Every member is one gzip member with the BC
+ * extra subfield (BSIZE = member size - 1), one final DEFLATE block (dynamic Huffman codes, or stored when that is not
+ * larger), CRC32 and ISIZE; the members are written back to back into out (DEVICE, capacity n * 65536 bytes) and
+ * out_offsets (DEVICE int64 [n + 1]) receives their start offsets and, last, the total length.  The 28-byte EOF marker is
+ * the caller's.  workspace: DEVICE memory of b200_bgzf_workspace_bytes(in_bytes) bytes.  Byte-identical from run to run.
+ */
+#define B200_BGZF_MEMBER_INPUT 65280 /* htslib's BGZF_BLOCK_SIZE (0xff00): a stored member still fits in 64 KiB */
+size_t b200_bgzf_workspace_bytes(int64_t in_bytes);
+int b200_bgzf_compress(const uint8_t* in, int64_t in_bytes, uint8_t* out, int64_t* out_offsets, void* workspace,
+                       size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
