@@ -12,7 +12,9 @@
 //   * W_hh (this warpgroup's 64 rows x 384) stays in registers as A fragments for the whole kernel: 24 k16 steps x 4;
 //   * W_ih (192 x 384 = 144 KB) stays in shared memory as a no-swizzle K-major A operand;
 //   * x_t comes from the previous layer's output [tile][T][64][H] by TMA: six 64-chunk x 64-column boxes (8 KB, 128-byte
-//     swizzle) per step through a ring of RING boxes that the MMAs of the x product release one by one;
+//     swizzle) per step through a ring of RING boxes that the MMAs of the x product release one by one.  The ring holds
+//     half a step, so each step's last three boxes are loaded while its first three are consumed; the cluster pulls
+//     every box into L2 PREFETCH steps ahead, so that those loads wait on L2 and not on HBM;
 //   * A row m of warpgroup wg is unit 16 wg + 4 (m/16) + (m%8)/2 (CTA-local), gate 2 (m%2) + (m%16)/8: the two rows a thread
 //     holds are (i, f) of a unit in even quads and (g, o) of the same unit in the odd quad next to it.  One __shfl_xor(4)
 //     per value pair then gives every thread all four gates of 8 cells (even quads take the even chunk of each column pair,
@@ -20,7 +22,8 @@
 // Schedule of a step: the x product of step t (its operands do not depend on h), bias and fp16 rounding of it -- exactly
 // the GEMM epilogue, so the gate pre-activations are bit-identical to b200_gemm_fwd_ex + lstm_rec_tile -- then the wait
 // for h_{t-1}, the W_hh product from zero, and acc + float(gx) per gate as lstm_rec_tile does.  The x product runs while
-// the peers' blocks of h_{t-1} are still in flight.
+// the peers' blocks of h_{t-1} are still in flight.  y of step t-1 is written from this CTA's block of h_{t-1} in the h
+// tile while the W_hh product runs; only the last step writes y from the staging block.
 //
 // Operands: x [tiles][T][64][H] fp16; wih [4H][H] and bias [4H] rows in [unit][gate] order (the gx column order of the
 // unfused path); whh [4H][H] rows [unit/8][gate][unit%8]; y [tiles][T][64][H].
@@ -37,6 +40,7 @@ constexpr int KCH = H / 8;                           // 48 k-chunks of 16 bytes
 constexpr int KS = H / 16;                           // 24 k16 steps
 constexpr int XBOX = H / 64;                         // x boxes per step: 64 columns (128 bytes) x 64 chunks
 constexpr int RING = 3;
+constexpr int PREFETCH = 2;                          // steps of x pulled into L2 ahead of the step that reads them
 constexpr uint32_t XBOX_BYTES = NB * 128;            // 8192
 constexpr uint32_t W_BYTES = KCH * ROWS * 16;        // 147456
 constexpr uint32_t HT_BYTES = KCH * NB * 16;         // 49152
@@ -51,6 +55,12 @@ __device__ __forceinline__ void bulk_multicast(uint32_t dst, const void* gsrc, u
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;\n" ::
             "r"(dst), "l"(gsrc), "r"(bytes), "r"(bar), "h"(mask)
         : "memory");
+}
+// pull a box of the tensor into L2 ahead of its TMA load (no shared memory, no completion to wait for)
+__device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int c0, int c1) {
+    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];\n" ::"l"(reinterpret_cast<uint64_t>(tmap)),
+                 "r"(c0), "r"(c1)
+                 : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;\n" ::: "memory"); }
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory"); }
@@ -145,6 +155,11 @@ lstm_fused_tile_kernel(const __grid_constant__ CUtensorMap tma_x, const __half* 
     for (int step = 0; step < T; ++step) {
         const int t = reverse ? (T - 1 - step) : step;
         const int par = step & 1;
+        // L2 prefetch of x (see the header): CTA `rank` < XBOX pulls box `rank` of step + PREFETCH
+        if (tid == 32 && (int)rank < XBOX && step + PREFETCH < T) {
+            const int sp = step + PREFETCH;
+            tma_prefetch_l2_2d(&tma_x, (int)rank * 64, xrow0 + (reverse ? (T - 1 - sp) : sp) * NB);
+        }
         // x product: acc = W_ih rows . x_t^T, k ascending like the GEMM
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc[i] = 0.f;
@@ -185,6 +200,15 @@ lstm_fused_tile_kernel(const __grid_constant__ CUtensorMap tma_x, const __half* 
             for (int ks = 0; ks < KS; ++ks)   // one k16 step = two k-chunks
                 wgmma_m64n64k16_f16_rs(acc, wa[ks], db_h + (uint64_t)(ks * 2 * NB * 16 / 16));
             wg_commit();
+            // while the MMAs run: y of the previous step from this CTA's own block of h_{t-1} in the h tile, so that
+            // these stores are not in front of the fence that releases the staged block of h_t to its bulk copy
+            const int tp = reverse ? (T - step) : (step - 1);
+            for (int i = tid; i < (int)(BLK_BYTES / 16); i += THREADS) {
+                const int kc = i / NB, chunk = i % NB;
+                if (chunk < nb)
+                    *reinterpret_cast<uint4*>(y + ((size_t)tp * NB + chunk) * H + rank * UPC + kc * 8) =
+                        *reinterpret_cast<const uint4*>(smem + OFF_H + rank * BLK_BYTES + (uint32_t)i * 16);
+            }
             wg_wait<0>();
             wg_fence_regs(acc);
         }
@@ -215,9 +239,12 @@ lstm_fused_tile_kernel(const __grid_constant__ CUtensorMap tma_x, const __half* 
         unsigned char* stg = hx + (size_t)par * BLK_BYTES;
         for (int i = tid; i < (int)(BLK_BYTES / 16); i += THREADS) {
             const uint4 v = *reinterpret_cast<const uint4*>(smem + OFF_ST + (uint32_t)i * 16);
-            if (step + 1 < T) reinterpret_cast<uint4*>(stg)[i] = v;
-            const int kc = i / NB, chunk = i % NB;
-            if (chunk < nb) *reinterpret_cast<uint4*>(y + ((size_t)t * NB + chunk) * H + rank * UPC + kc * 8) = v;
+            if (step + 1 < T) {
+                reinterpret_cast<uint4*>(stg)[i] = v;
+            } else {   // the last step's h_t is not exchanged: y straight from the staged block
+                const int kc = i / NB, chunk = i % NB;
+                if (chunk < nb) *reinterpret_cast<uint4*>(y + ((size_t)t * NB + chunk) * H + rank * UPC + kc * 8) = v;
+            }
         }
         if (step + 1 == T) break;
         fence_proxy_async_global();   // the staged block (generic stores) -> visible to the bulk copy (async proxy)
