@@ -4,8 +4,11 @@
 Output is FASTQ, or SAM text with the `mv:B:c` move table when stdout is redirected to a `.sam` file, or BAM with the same
 records when it is redirected to a `.bam` file, BGZF-compressed on the GPU (the reference's `biofmt` rule,
 bonito/io.py:35-54); CRAM is refused.  `--reference <fasta>` maps the calls on the GPU (bonito_b200.aligner, this
-project's rules in place of minimap2's) and writes aligned SAM or BAM; `--alignment-threads` is accepted and has no effect.  CTC
-training-data export (`--save-ctc`) exits with an explanation.
+project's rules in place of minimap2's) and writes aligned SAM or BAM; `--alignment-threads` is accepted and has no effect.
+`--reference <fasta> --save-ctc` writes CTC training data (the reference's `--save-ctc`, bonito/cli/basecaller.py:118-154):
+each read is cut into model-sized chunks (bonito_b200.reader.read_chunks), every chunk is basecalled and mapped as a read
+of its own, and bonito_b200.io.CtcWriter filters them and saves `chunks.npy`, `references.npy`, `reference_lengths.npy`
+and a summary TSV beside the stdout file, with the kept chunks' records on stdout (its docstring lists the deviations).
 `B200_CTC_BEAMSIZE=W` in the environment (1..32, unset = 1, the greedy decode) decodes the QuartzNet CTC models with the
 prefix beam search of width W; the flag surface itself is the reference's and has no beam option.
 """
@@ -21,9 +24,9 @@ import numpy as np
 
 from bonito_b200.aligner import PRESETS, Aligner, IndexBuildError, align_map
 from bonito_b200.ctc.model import MAX_BEAMSIZE, Model as CtcModel
-from bonito_b200.io import BamWriter, Writer, biofmt
+from bonito_b200.io import BamWriter, CtcDataError, CtcWriter, Writer, biofmt
 from bonito_b200.nn import fuse_bn_
-from bonito_b200.reader import Reader
+from bonito_b200.reader import Reader, read_chunks
 from bonito_b200.util import init, load_model, load_symbol
 
 
@@ -36,8 +39,8 @@ def _column_to_set(filename, idx=0):
 
 def main(args):
     init(args.seed, args.device)
-    if args.save_ctc:
-        sys.stderr.write("> error: --save-ctc (CTC training data) is not supported by this build\n")
+    if args.save_ctc and not args.reference:
+        sys.stderr.write("> error: --save-ctc needs --reference: a reference is needed to output ctc training data\n")
         exit(1)
     if args.reference and args.mm2_preset not in PRESETS:
         sys.stderr.write(f"> error: unknown --mm2-preset '{args.mm2_preset}', choose one of {', '.join(PRESETS)}\n")
@@ -90,7 +93,8 @@ def main(args):
 
     basecall = load_symbol(args.model_directory, "basecall")
     aligner = None
-    if args.reference and fmt.name != "fastq":       # FASTQ has no alignment fields: the mapping is skipped
+    # FASTQ has no alignment fields, so plain `--reference` skips the mapping there; CTC training data always needs it
+    if args.reference and (fmt.name != "fastq" or args.save_ctc):
         sys.stderr.write("> loading reference\n")
         try:
             aligner = Aligner(args.reference, preset=args.mm2_preset, device=args.device)
@@ -107,13 +111,18 @@ def main(args):
         reads = islice(reads, args.max_reads)
 
     params = model.config["basecaller"]
+    if args.save_ctc:
+        reads = (chunk for read in reads for chunk in read_chunks(read, params["chunksize"], params["overlap"]))
     results = basecall(model, reads, reverse=args.revcomp, rna=args.rna, batchsize=params["batchsize"],
                        chunksize=params["chunksize"], overlap=params["overlap"], **decode_args)
     if aligner:
         results = align_map(aligner, results, n_thread=args.alignment_threads)
     writer_args = dict(min_qscore=args.min_qscore, group_key=os.path.basename(os.path.normpath(args.model_directory)),
                        contigs=aligner.contigs if aligner else None)
-    if fmt.mode == "wb":
+    if args.save_ctc:
+        writer = CtcWriter(results, aligner, mode=fmt.mode, min_qscore=args.min_qscore,
+                           min_accuracy=args.min_accuracy_save_ctc, rna=args.rna, device=args.device)
+    elif fmt.mode == "wb":
         writer = BamWriter(results, device=args.device, **writer_args)
     else:
         writer = Writer(results, mode=fmt.mode, **writer_args)
@@ -121,6 +130,9 @@ def main(args):
     writer.start()
     writer.join()
     duration = perf_counter() - t0
+    if isinstance(writer.error, CtcDataError):
+        sys.stderr.write(f"> error: {writer.error}\n")
+        exit(1)
     if writer.error is not None:
         raise writer.error
     num_samples = sum(n for _, n in writer.log)

@@ -7,9 +7,25 @@ builds (bonito_b200.bam), BGZF-compressed on the GPU; CRAM needs htslib, which t
 with an explanation instead of being approximated.
 Deviation: on the reverse strand QUAL is reversed along with SEQ, as the SAM specification requires; the reference
 reverse-complements SEQ and leaves QUAL as called.
+
+`CtcWriter` writes the CTC training data of `basecaller --reference --save-ctc` (reference: `CTCWriter`,
+bonito/io.py:513-619): every mapped chunk call that passes the reference's filters becomes a row of `chunks.npy`,
+`references.npy` and `reference_lengths.npy`, and a record on stdout.  Deviations from the reference:
+  * when every target has the same length (sd = 0) `typical_indices` keeps all rows; the reference's strict
+    `mu - 2.5 sd < x < mu + 2.5 sd` keeps none and then reports success with empty arrays.
+  * a Mapping has no `mlen` / `blen`: they come from its CIGAR (M / I / D) and NM, `blen = M + I + D`, `mlen = blen - NM`,
+    so N columns count in both (mappy leaves ambiguous bases out).  A chunk over an N is rejected either way; only the
+    reject name can differ.
+  * the summary TSV is overwritten; the reference's CSVLogger appends to an existing file and then rewrites it.
+  * a target over 65 535 bases stops the run with an error instead of wrapping in uint16 (only a very large
+    `--chunksize` can produce one).
+  * the arrays and summary go next to the file stdout is redirected to, or to the working directory when stdout is not a
+    regular file (a terminal, a pipe, /dev/null); the reference's `dirname(realpath('/dev/fd/1'))` points into /proc for
+    a pipe.
 """
 
 import os
+import re
 import sys
 from collections import namedtuple
 from os.path import realpath
@@ -247,3 +263,223 @@ class BamWriter(Writer):
 
     def end(self):
         self.bam.close()
+
+
+summary_field_names = [
+    "filename", "read_id", "run_id", "channel", "mux", "start_time", "duration", "template_start", "template_duration",
+    "sequence_length_template", "mean_qscore_template",
+    "alignment_genome", "alignment_genome_start", "alignment_genome_end", "alignment_strand_start",
+    "alignment_strand_end", "alignment_direction", "alignment_length", "alignment_num_aligned", "alignment_num_correct",
+    "alignment_num_insertions", "alignment_num_deletions", "alignment_num_substitutions", "alignment_mapq",
+    "alignment_strand_coverage", "alignment_identity", "alignment_accuracy",
+]
+
+_CIGAR_OP = re.compile(r"(\d+)([MID])")
+_TARGET_CODE = np.zeros(256, dtype=np.uint8)
+_TARGET_CODE[np.frombuffer(b"ACGT", dtype=np.uint8)] = np.arange(1, 5, dtype=np.uint8)
+MAX_TARGET = np.iinfo(np.uint16).max
+
+
+class CtcDataError(ValueError):
+    """CTC training data that cannot be written as the reference's dtypes (a target longer than uint16 counts)."""
+
+
+def cigar_counts(cigar_str):
+    """(M, I, D) base counts of an M / I / D CIGAR string."""
+    counts = {"M": 0, "I": 0, "D": 0}
+    for n, op in _CIGAR_OP.findall(cigar_str):
+        counts[op] += int(n)
+    return counts["M"], counts["I"], counts["D"]
+
+
+def alignment_lengths(mapping):
+    """(mlen, blen) of a Mapping as mappy defines them, from its CIGAR and NM: blen = M + I + D, mlen = blen - NM."""
+    blen = sum(cigar_counts(mapping.cigar_str))
+    return blen - mapping.NM, blen
+
+
+def summary_row(read, seqlen, qscore, mapping):
+    """One row of the summary TSV, a dict keyed by `summary_field_names` (reference: bonito/io.py:211-258)."""
+    fields = [read.filename, read.read_id, read.run_id, read.channel, read.mux, read.start, read.duration,
+              read.template_start, read.template_duration, seqlen, float(qscore)]
+    if mapping is None:
+        fields += ["*", -1, -1, -1, -1, "*", 0, 0, 0, 0, 0, 0, 0, 0.0, 0.0, 0.0]
+    else:
+        _, ins, dels = cigar_counts(mapping.cigar_str)
+        correct, length = alignment_lengths(mapping)
+        matches = length - ins - dels
+        fwd = mapping.strand == +1
+        fields += [mapping.ctg, mapping.r_st, mapping.r_en,
+                   mapping.q_st if fwd else seqlen - mapping.q_en, mapping.q_en if fwd else seqlen - mapping.q_st,
+                   "+" if fwd else "-", length, matches, correct, ins, dels, mapping.NM - ins - dels, mapping.mapq,
+                   (mapping.q_en - mapping.q_st) / seqlen, correct / matches if matches else 0.0,
+                   correct / length if length else 0.0]
+    return dict(zip(summary_field_names, fields))
+
+
+def typical_indices(x, n=2.5):
+    """Indices of the values strictly within n standard deviations of the mean (reference: bonito/io.py:29-32).
+    Deviation: when every value is the same (sd = 0) all indices are kept; the reference's strict test keeps none."""
+    x = np.asarray(x)
+    mu, sd = np.mean(x), np.std(x)
+    if sd == 0:
+        return np.arange(x.size)
+    idx, = np.where((mu - n * sd < x) & (x < mu + n * sd))
+    return idx
+
+
+def ctc_target(refseq, strand, rna=False):
+    """uint8 target of a reference span: reverse-complemented on strand -1, A C G T -> 1 2 3 4, reversed back to signal
+    orientation for RNA (whose calls are reversed)."""
+    if strand == -1:
+        refseq = revcomp(refseq)
+    target = _TARGET_CODE[np.frombuffer(refseq.encode(), dtype=np.uint8)]
+    return target[::-1].copy() if rna else target
+
+
+def ctc_reject(seq, mean_qscore, mapping, refseq, min_qscore=0, min_accuracy=0.99, min_coverage=0.90):
+    """The reject name of a chunk call, the first of the reference's filters that holds in its order, or None when the
+    chunk is kept.  `refseq` is the mapped reference span (unused when `mapping` is None)."""
+    if mean_qscore < min_qscore:
+        return "low_qscore"
+    if not len(seq):
+        return "zerolen_sequence"
+    if mapping is None:
+        return "no_mapping"
+    mlen, blen = alignment_lengths(mapping)
+    if (mlen / blen if blen else 0.0) < min_accuracy:
+        return f"low_accuracy{min_accuracy:.2f}"
+    if (mapping.q_en - mapping.q_st) / len(seq) < min_coverage:
+        return f"low_coverage{min_coverage:.2f}"
+    if "N" in refseq:
+        return "N_in_sequence"
+    return None
+
+
+def ctc_output_paths(fd=1):
+    """(directory, summary file) of the CTC training data: beside the regular file `fd` is redirected to, as
+    `<stem>_summary.tsv`; otherwise (a terminal, a pipe, a device) the working directory and `summary.tsv`."""
+    path = ""
+    if not os.isatty(fd):
+        try:
+            path = realpath(f"/dev/fd/{fd}")
+        except OSError:
+            path = ""
+    if path and not path.startswith("/proc") and os.path.isfile(path):
+        return os.path.dirname(path), "%s_summary.tsv" % os.path.splitext(path)[0]
+    return ".", "summary.tsv"
+
+
+def _tsv_value(v):
+    return repr(v) if isinstance(v, float) else str(v)
+
+
+def write_summary(path, rows):
+    """The summary TSV: a header line of `summary_field_names`, then one line per row dict."""
+    with open(path, "w") as fh:
+        fh.write("\t".join(summary_field_names) + "\n")
+        for row in rows:
+            fh.write("\t".join(_tsv_value(row[k]) for k in summary_field_names) + "\n")
+
+
+class CtcWriter(Thread):
+    """
+    Writes the CTC training data of `basecaller --save-ctc` from (chunk read, result with `mapping`) pairs.  `aligner` is
+    any object with `seq(name, start, end)` and `contigs` [(name, length)].  Chunks are filtered by `ctc_reject`; every
+    kept chunk is written to `fd` in input order as a record without tags: SAM text with the header in mode "w", BAM
+    (BGZF on `device`) in mode "wb", SAM lines without a header in mode "wfq" (the reference's pysam output with
+    `add_sam_header=False`).  At the end the rows within `typical_indices` of the target lengths are saved in the order of
+    `np.random.permutation` (numpy's global state, seeded by `init`) to `chunks.npy` (float16 [n, chunksize]),
+    `references.npy` (uint8 [n, max length], zero-padded) and `reference_lengths.npy` (uint16 [n]) in `directory`, with
+    the summary TSV `summary` filtered and permuted in step.  `.log` holds (chunk id, samples) of every chunk; `.rejected`
+    the reject counts in order of first occurrence.
+    """
+
+    def __init__(self, iterator, aligner, fd=None, mode="w", min_qscore=0, min_accuracy=0.99, min_coverage=0.90,
+                 rna=False, directory=None, summary=None, device="cuda", stderr=None):
+        super().__init__(daemon=True)
+        if mode not in ("wfq", "w", "wb"):
+            raise ValueError(f"output mode {mode!r} needs htslib (CRAM), which this build does not bundle: "
+                             "redirect to a .bam, .sam or .fastq file")
+        if fd is None:
+            fd = sys.stdout.buffer if mode == "wb" else sys.stdout
+        if directory is None or summary is None:
+            default_dir, default_summary = ctc_output_paths()
+            directory = default_dir if directory is None else directory
+            summary = default_summary if summary is None else summary
+        self.iterator, self.aligner, self.fd, self.mode = iterator, aligner, fd, mode
+        self.min_qscore, self.min_accuracy, self.min_coverage, self.rna = min_qscore, min_accuracy, min_coverage, rna
+        self.directory, self.summary = directory, summary
+        self.device = device
+        self.stderr = stderr if stderr is not None else sys.stderr
+        self.log, self.rejected, self.error = [], {}, None
+
+    def run(self):
+        try:
+            self.begin()
+            chunks, targets, rows = [], [], []
+            for read, res in self.iterator:
+                seq, qstring = res["sequence"], res["qstring"]
+                mean_qscore = res.get("mean_qscore", mean_qscore_from_qstring(qstring))
+                mapping = res.get("mapping")
+                self.log.append((read.read_id, len(read.signal)))
+                refseq = self.aligner.seq(mapping.ctg, mapping.r_st, mapping.r_en) if mapping and len(seq) else ""
+                reason = ctc_reject(seq, mean_qscore, mapping, refseq, self.min_qscore, self.min_accuracy,
+                                    self.min_coverage)
+                if reason is not None:
+                    self.rejected[reason] = self.rejected.get(reason, 0) + 1
+                    continue
+                target = ctc_target(refseq, mapping.strand, self.rna)
+                if target.size > MAX_TARGET:
+                    raise CtcDataError(f"chunk {read.read_id} has a {target.size}-base reference, over the {MAX_TARGET} "
+                                       "that reference_lengths.npy (uint16) holds: use a smaller --chunksize")
+                self.write_record(sam_record(read.read_id, seq, qstring, mapping))
+                rows.append(summary_row(read, len(seq), mean_qscore, mapping))
+                targets.append(target)
+                chunks.append(np.asarray(read.signal, dtype=np.float16))
+            self.end()
+            self.save(chunks, targets, rows)
+        except BaseException as err:   # surfaced by the CLI after join()
+            self.error = err
+
+    def begin(self):
+        header = sam_header(contigs=self.aligner.contigs)
+        if self.mode == "wb":
+            self.bam = BamOutput(self.fd, header, self.aligner.contigs, device=self.device)
+        elif self.mode == "w":
+            self.fd.write(header)
+
+    def write_record(self, line):
+        if self.mode == "wb":
+            self.bam.write_sam(line)
+        else:
+            self.fd.write(line + "\n")
+
+    def end(self):
+        if self.mode == "wb":
+            self.bam.close()
+        else:
+            self.fd.flush()
+
+    def save(self, chunks, targets, rows):
+        if not chunks:
+            self.stderr.write("> no suitable ctc data to write\n")
+            return
+        chunks = np.stack(chunks)
+        lengths = np.array([t.size for t in targets], dtype=np.uint16)
+        references = np.zeros((len(targets), int(lengths.max())), dtype=np.uint8)
+        for row, target in zip(references, targets):
+            row[:target.size] = target
+        indices = np.random.permutation(typical_indices(lengths))
+        chunks, references, lengths = chunks[indices], references[indices], lengths[indices]
+        write_summary(self.summary, [rows[i] for i in indices])
+        np.save(os.path.join(self.directory, "chunks.npy"), chunks)
+        np.save(os.path.join(self.directory, "references.npy"), references)
+        np.save(os.path.join(self.directory, "reference_lengths.npy"), lengths)
+        self.stderr.write("> Chunks rejected from training data:\n")
+        for name, count in self.rejected.items():
+            self.stderr.write(f" - {name}: {count}\n")
+        self.stderr.write(f"> written ctc training data to {self.directory}\n")
+        self.stderr.write("  - chunks.npy with shape (%s)\n" % ",".join(map(str, chunks.shape)))
+        self.stderr.write("  - references.npy with shape (%s)\n" % ",".join(map(str, references.shape)))
+        self.stderr.write("  - reference_lengths.npy shape (%s)\n" % ",".join(map(str, lengths.shape)))

@@ -86,6 +86,41 @@ class Read:
                 f"sv:Z:{self.scaling_strategy}"]
 
 
+class ReadChunk:
+    """One fixed-size window of a read, basecalled as a read of its own for `basecaller --save-ctc` (reference:
+    bonito/reader.py:89-104): named `<read_id>:<i>:<n>`, with the parent's metadata and `template_start` /
+    `template_duration` set to the parent's start time and duration."""
+
+    def __init__(self, read, chunk, i, n):
+        self.read_id = f"{read.read_id}:{i}:{n}"
+        self.filename, self.run_id, self.mux, self.channel = read.filename, read.run_id, read.mux, read.channel
+        self.read_number, self.shift, self.scale = read.read_number, read.shift, read.scale
+        self.scaling_strategy = read.scaling_strategy
+        self.start, self.duration = read.start_time, read.duration
+        self.template_start, self.template_duration = self.start, self.duration
+        self.signal = chunk
+
+    def __repr__(self):
+        return f"ReadChunk('{self.read_id}')"
+
+
+def read_chunks(read, chunksize=4000, overlap=400):
+    """
+    The read's (already trimmed and normalised) signal cut into `chunksize` windows `chunksize - overlap` apart, as
+    ReadChunks (reference: bonito/reader.py:107-119).  A read shorter than a chunk gives none; otherwise the first
+    `(len - chunksize) % (chunksize - overlap)` samples are dropped, so the last window ends at the read's end.
+    """
+    length = len(read.signal)
+    if length < chunksize:
+        return
+    step = chunksize - overlap
+    offset = (length - chunksize) % step
+    n = (length - offset - chunksize) // step + 1
+    for i in range(n):
+        start = offset + i * step
+        yield ReadChunk(read, read.signal[start:start + chunksize], i + 1, n)
+
+
 class Reader:
     def __init__(self, directory, recursive=False):
         self.fmt = None
