@@ -60,6 +60,7 @@ int launch_crf_beam_search(const __half* scores, int N, int T, int state_len, fl
                            float qbias, void* workspace, uint8_t* moves, uint8_t* seq, uint8_t* qual, cudaStream_t stream);
 
 int launch_lstm_crf_fwd(const b200_lstm_crf_plan* p, const __half* x, __half* scores, cudaStream_t stream);
+int launch_lstm_stack(const b200_lstm_crf_plan* p, int first, int count, cudaStream_t stream);
 
 size_t ctc_crf_sparse_workspace_bytes(int N, int T, int state_len, int semiring);
 size_t ctc_crf_target_workspace_bytes(int N, int T, int L, int semiring);
@@ -374,6 +375,11 @@ int b200_gemm_i8_fwd(const void* a, long long lda, const void* b, const void* co
 
 int b200_lstm_crf_fwd(const b200_lstm_crf_plan* plan, const void* x, void* scores, void* stream) {
     return launch_lstm_crf_fwd(plan, (const __half*)x, (__half*)scores, (cudaStream_t)stream);
+}
+
+int b200_lstm_crf_lstm_fwd(const b200_lstm_crf_plan* plan, int first, int count, void* stream) {
+    B200_REQUIRE(plan != nullptr, "lstm_crf_lstm: null plan");
+    return launch_lstm_stack(plan, first, count, (cudaStream_t)stream);
 }
 
 int b200_crf_beam_search(const void* scores, int n, int t, int state_len, float blank_score, int beam_width, float beam_cut,

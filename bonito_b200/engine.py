@@ -22,9 +22,10 @@ more GEMM; these layers and learned blank scores run on the wide layout (H = 768
 Every layout shares the front end: the fused conv1 + conv2 stem writes `[N][Lp][C2]` channels last, and the strided conv3 is
 one GEMM over the overlapping-row view of it.  The LSTM width picks one of three activation layouts (`LstmCrfPlan.forward`):
 
-* Tile layout, width 384 (hac, the headline path; `forward_tiles`): activations tile-major `[tile][T][64][H]`; layer by
-  layer on the current stream, per layer ONE launch of the fused wgmma LSTM kernel (lstm_fused_tile.cu: one 8-CTA cluster
-  per 64-chunk tile, 8 clusters for 512 chunks), which computes the input projection inside the recurrence.  Under
+* Tile layout, width 384 (hac, the headline path; `forward_tiles`): activations tile-major `[tile][T][64][H]`; the fused
+  wgmma LSTM kernel (lstm_fused_tile.cu: one 8-CTA cluster per 64-chunk tile, 8 clusters for 512 chunks), which computes
+  the input projection inside the recurrence, runs the LSTM stack in chains of consecutive tiles, each chain on a stream
+  of its own through all the layers (b200_lstm_crf_lstm_fwd).  Under
   `--quantize` the input projection is an int8 GEMM into gate pre-activations `[tile][T][8][64][192]` instead, followed by
   the unfused recurrent kernel (lstm_rec_tile.cu).  The whole encoder is one C call (`b200_lstm_crf_fwd`) unless per-kernel
   events, intermediate activations, another GEMM implementation or the int8 input projection ask for the launches one at
@@ -223,6 +224,8 @@ class LstmCrfPlan:
                 self.lstm[-1]["wih_q"] = torch.round(w / s_w[:, None]).clamp(-127, 127).to(torch.int8).to(device).contiguous()
                 self.lstm[-1]["wih_scale"] = (s_w / 127.0).to(device=device, dtype=torch.float32).contiguous()
         self.quantize = bool(quantize)
+        if self.tile and len(self.lstm) > native.MAX_LSTM_LAYERS:
+            raise UnsupportedModel(f"the tile-layout LSTM path runs at most {native.MAX_LSTM_LAYERS} layers; got {len(self.lstm)}")
         if self.quantize and not (self.tile and H % 16 == 0):
             raise UnsupportedModel("the int8 input projection (--quantize) needs the tile-layout LSTM path (hidden size 384)")
 
@@ -268,6 +271,7 @@ class LstmCrfPlan:
         else:
             self.act_l, self.lo, self.hi = crf_act, 0.0, 0.0
         self._bufs = {}
+        self._chain_streams = {}    # slot -> streams of the LSTM stack's tile chains 1.. (b200_lstm_crf_lstm_fwd)
         self._wide_pending = None   # (event, pinned status words) of the last wide-path forward, checked by the next call
 
     # ------------------------------------------------------------------------------------------
@@ -318,6 +322,9 @@ class LstmCrfPlan:
                 yq=torch.empty(nt * T * TB * H, dtype=torch.int8, device=dev) if self.quantize else None,
                 # staging of the recurrent kernel's h all-gather: one region per tile (the clusters run concurrently)
                 hx=torch.empty(nt, native.lstm_rec_tile_workspace_bytes(TB), dtype=torch.uint8, device=dev),
+                # kept per slot for the life of the plan: a buffer set of another geometry reuses them
+                chains=self._chain_streams.setdefault(
+                    slot, [native.new_stream(dev) for _ in range(native.LSTM_CHAINS - 1)]),
             )
         else:
             ws = torch.empty(native.lstm_rec_wide_workspace_bytes(N, H), dtype=torch.uint8, device=dev)
@@ -439,14 +446,17 @@ class LstmCrfPlan:
                 p.reverse[i] = int(layer["reverse"])
                 p.wih[i], p.bias[i], p.whh[i] = ptr(layer["wih"]), ptr(layer["bias"]), ptr(layer["whh"])
             p.stem, p.ya, p.yb, p.gx, p.hx = (ptr(b[k]) for k in ("stem", "ya", "yb", "gx", "hx"))
+            for i, st in enumerate(b["chains"]):
+                p.chain_streams[i] = st.cuda_stream
             b["struct"] = p
         return b["struct"]
 
     def forward_tiles(self, x, out=None, gemm_impl=native.GEMM_AUTO, events=None, return_features=False, slot=0):
         """
-        Forward in the tile layout, layer by layer on the current stream: ONE launch of the fused LSTM kernel (a cluster per
-        tile, all in one wave) per layer, or the int8 input-projection GEMM and the recurrent kernel under `quantize`.  `slot` selects one of several independent buffer sets (batches in
-        flight at the same time).
+        Forward in the tile layout: the fused LSTM kernel over the whole stack in chains of tiles, each chain on a stream of
+        its own (b200_lstm_crf_lstm_fwd), or layer by layer on the current stream the int8 input-projection GEMM and the
+        recurrent kernel under `quantize`.  `slot` selects one of several independent buffer sets (batches in flight at
+        the same time), each with its own chain streams.
         """
         x = self._input(x)
         N, L = x.shape
@@ -474,8 +484,8 @@ class LstmCrfPlan:
         if feats is not None:
             feats["conv"] = gather(cur)
         rows = dict(rows_inner=TB, valid_inner=TB, stride_inner=1, stride_outer=CS * TB, cb_width=CW, cb_rows=TB)
-        for li, layer in enumerate(self.lstm):
-            if self.quantize:
+        if self.quantize:
+            for li, layer in enumerate(self.lstm):
                 # rows (tile, t, chunk) -> gx[tile][t][rank][chunk][CW]
                 with _Stage("quantize_i8", events):
                     native.quantize_i8(cur, b["yq"], 127.0)
@@ -484,13 +494,19 @@ class LstmCrfPlan:
                                    4 * H, H, **rows)
                 with _Stage("lstm_rec", events):
                     native.lstm_rec_tile(b["gx"], layer["whh"], nxt, T, N, H, layer["reverse"], workspace=b["hx"])
-            else:
+                cur, nxt = nxt, cur
+                if feats is not None:
+                    feats[f"lstm{li}"] = gather(cur)
+        else:
+            # the stack as b200_lstm_crf_fwd runs it (chains of tiles on the slot's chain streams); layer by layer when the
+            # activations between layers are wanted
+            n = len(self.lstm)
+            for first, count in ([(i, 1) for i in range(n)] if feats is not None else [(0, n)]):
                 with _Stage("lstm_rec", events):
-                    native.lstm_fused_tile(cur, layer["wih"], layer["bias"], layer["whh"], nxt, T, N, H, layer["reverse"],
-                                           workspace=b["hx"])
-            cur, nxt = nxt, cur
-            if feats is not None:
-                feats[f"lstm{li}"] = gather(cur)
+                    native.lstm_crf_lstm_fwd(self._plan_struct(b, N, L), first, count)
+                if feats is not None:
+                    feats[f"lstm{first}"] = gather(b["ya"] if first % 2 else b["yb"])
+            cur = b["yb"] if n % 2 else b["ya"]
         # full tiles in one launch: rows r = (tile*T + t)*TB + i -> out[tile*TB + i][t]; a last tile the batch does not fill
         # in a launch of its own, whose `valid_inner` cuts off the rows of chunks beyond the batch
         full = N // TB

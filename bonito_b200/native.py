@@ -20,6 +20,7 @@ ACT_NONE, ACT_SWISH, ACT_TANH, ACT_CLAMP, ACT_SCALE, ACT_SWIGLU, ACT_TANH_SCALE,
 GEMM_AUTO, GEMM_TCGEN05, GEMM_MMA_SYNC = 0, 1, 2
 
 MAX_LSTM_LAYERS = 8
+LSTM_CHAINS = 4
 
 
 class LstmCrfPlanStruct(ctypes.Structure):
@@ -33,7 +34,8 @@ class LstmCrfPlanStruct(ctypes.Structure):
                 ("w1", c_void_p), ("b1", c_void_p), ("w2", c_void_p), ("b2", c_void_p), ("w3", c_void_p), ("b3", c_void_p),
                 ("wl", c_void_p), ("bl", c_void_p),
                 ("wih", c_void_p * MAX_LSTM_LAYERS), ("bias", c_void_p * MAX_LSTM_LAYERS), ("whh", c_void_p * MAX_LSTM_LAYERS),
-                ("stem", c_void_p), ("ya", c_void_p), ("yb", c_void_p), ("gx", c_void_p), ("hx", c_void_p)]
+                ("stem", c_void_p), ("ya", c_void_p), ("yb", c_void_p), ("gx", c_void_p), ("hx", c_void_p),
+                ("chain_streams", c_void_p * (LSTM_CHAINS - 1))]
 
 
 # name -> (restype, argtypes); must list every symbol declared in include/bonito_b200.h
@@ -90,6 +92,7 @@ SIGNATURES = {
                                  c_int, c_float, c_float, c_int, c_int, c_longlong, c_longlong, c_int, c_longlong, c_int, c_int,
                                  c_int, c_void_p]),
     "b200_lstm_crf_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_lstm_crf_lstm_fwd": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "b200_crf_beam_search": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_int, c_float, c_float, c_float,
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200_crf_decode": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_float, c_float,
@@ -712,6 +715,13 @@ def chunk_signal(signal, chunksize, overlap, out=None, stream=None):
                                    _ptr(out), int(chunksize), _stream(stream))
     _check(rc, "b200_chunk_signal")
     return out
+
+
+def lstm_crf_lstm_fwd(plan_struct, first, count, stream=None):
+    """LSTM layers [first, first + count) of a filled LstmCrfPlanStruct, in chains of tiles (see b200_lstm_crf_lstm_fwd)."""
+    lib = require()
+    rc = lib.b200_lstm_crf_lstm_fwd(ctypes.byref(plan_struct), int(first), int(count), _stream(stream))
+    _check(rc, "b200_lstm_crf_lstm_fwd")
 
 
 def new_stream(device):

@@ -342,8 +342,9 @@ int b200_gemm_i8_fwd(const void* a, long long lda, const void* b, const void* co
 
 /*
  * ---- coarse entry point: the whole LSTM-CRF encoder forward of one batch from one call ----
- * conv stem -> strided convolution (GEMM) -> n_lstm x fused LSTM layer (b200_lstm_fused_tile_fwd) -> LinearCRFEncoder
- * GEMM (+Clamp), enqueued on `stream` (9 launches for the hac shape).  Replaces the module-tree walk of
+ * conv stem -> strided convolution (GEMM) -> n_lstm x fused LSTM layer (b200_lstm_fused_tile_fwd, in chains of tiles on
+ * `stream` and the plan's chain_streams, see b200_lstm_crf_lstm_fwd) -> LinearCRFEncoder GEMM (+Clamp), enqueued on
+ * `stream`.  Replaces the module-tree walk of
  * `Serial.forward` over the encoder of a bonito.crf model (bonito/nn.py:82-89, bonito/crf/model.py:150-162) -- the span
  * `Model.use_koi` swaps for koi.lstm.update_graph plus the layers around it.  Tile-layout recurrent kernel only
  * (b200_lstm_tile_chunks(hidden) > 0).  The plan holds DEVICE pointers to packed weights (layouts as documented for the
@@ -355,6 +356,8 @@ int b200_gemm_i8_fwd(const void* a, long long lda, const void* b, const void* co
  * x [n][l] fp16 -> scores [n][t][n_scores] fp16 (no blank column).
  */
 #define B200_MAX_LSTM_LAYERS 8
+/* chains of tiles the LSTM stack of b200_lstm_crf_fwd is split into (see b200_lstm_crf_lstm_fwd) */
+#define B200_LSTM_CHAINS 4
 typedef struct b200_lstm_crf_plan {
     int n, l, t, tp;
     int c1, k1, act1, c2, k2, act2;          /* conv stem */
@@ -367,8 +370,19 @@ typedef struct b200_lstm_crf_plan {
     const void* bias[B200_MAX_LSTM_LAYERS];
     const void* whh[B200_MAX_LSTM_LAYERS];
     void *stem, *ya, *yb, *gx, *hx;
+    /* B200_LSTM_CHAINS - 1 caller-owned streams (cudaStream_t, NULL: none) for the chains of tiles of the LSTM stack */
+    void* chain_streams[B200_LSTM_CHAINS - 1];
 } b200_lstm_crf_plan;
 int b200_lstm_crf_fwd(const b200_lstm_crf_plan* plan, const void* x, void* scores, void* stream);
+
+/*
+ * LSTM layers [first, first + count) of the plan (layer i reads ya when i is even, yb when odd, and writes the other), as
+ * b200_lstm_crf_fwd runs them: the tiles are split into up to B200_LSTM_CHAINS chains of consecutive tiles, chain 0 on
+ * `stream` and chain c on chain_streams[c - 1] (chains without a stream are not formed), each running its tiles through
+ * the layers as one launch of the fused kernel per layer.  The chains start after the work enqueued on `stream` so far
+ * and the work enqueued on `stream` afterwards waits for all of them.  Results are those of one launch per layer.
+ */
+int b200_lstm_crf_lstm_fwd(const b200_lstm_crf_plan* plan, int first, int count, void* stream);
 
 /*
  * Beam-search decode with the argument meaning of koi.decode.beam_search (bonito/crf/basecall.py:36-40): beam_width entries

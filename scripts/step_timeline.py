@@ -1,6 +1,6 @@
 """Launch-level timeline of the pipelined hac step (two batches in flight): start / end of every kernel of a few steady-state
-steps, by stream, from the CUDA events the engine records per launch, and the time of each LSTM layer's recurrent launch
-(`lstm_rec`: the whole layer when the input projection is fused in) per layer and per time step."""
+steps, by stream, from the CUDA events the engine records per launch, and the time of the LSTM stack (`lstm_rec`: all
+layers, in chains of tiles, when the input projection is fused in) per step and per time step and layer."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -49,8 +49,7 @@ for a, b, i, name in sorted(rows):
     if i in (4, 5, 6):
         print(f"step {i} (stream {i % SLOTS})  {name:14s} {a - lo:8.2f} -> {b - lo:8.2f}   {b - a:6.2f} ms")
 T = plan.frames(L)
-rec = [[b - a for a, b, i, name in sorted(rows) if i == s and name == "lstm_rec"] for s in range(4, 8)]
-for layer in range(len(rec[0])):
-    ms = [r[layer] for r in rec]
-    print(f"lstm_rec layer {layer}: {min(ms):6.2f} .. {max(ms):6.2f} ms over steps 4-7, "
-          f"{1e3 * sum(ms) / len(ms) / T:5.2f} us per time step ({T} steps)")
+n_layers = len(plan.lstm)
+rec = [sum(b - a for a, b, i, name in rows if i == s and name == "lstm_rec") for s in range(4, 8)]
+print(f"lstm_rec (the {n_layers}-layer stack): {min(rec):6.2f} .. {max(rec):6.2f} ms per step over steps 4-7, "
+      f"{1e3 * sum(rec) / len(rec) / T / n_layers:5.2f} us per time step and layer ({T} steps)")
