@@ -1,19 +1,25 @@
 // C[M,N] = epilogue(A[M,K] * B[N,K]^T) on the Hopper tensor cores (wgmma, sm_90a): the product GEMM of every
 // convolution-as-GEMM, LSTM input projection, CRF head and transformer projection.
 //
-//   * a CTA owns one 128-row block of A and sweeps a run of 128-column tiles of N (all of them when the grid is large
-//     enough), so that one CTA streams tile after tile through one pipeline: while it rounds and stores tile j, the next
-//     tile's operands are already arriving;
+//   * a CTA owns one 128-row block of A and sweeps a run of up to MAX_RUN 128-column tiles of N through one pipeline:
+//     while it rounds and stores tile j, the next tile's operands are already arriving.  The runs of a row block are
+//     consecutive CTAs, so they are resident together: they read the same A rows from L2 and write neighbouring parts
+//     of the same output rows;
 //   * one producer warp fills a 3-deep ring of stages with TMA copies (128-byte K slices -- 64 fp16 or 128 int8 -- of 128
 //     rows of A and of B, 128-byte swizzle), signalling through mbarriers ("full": bytes landed, "empty": every consumer
 //     warp is done with the stage);
 //   * two consumer warpgroups of 64 rows each issue wgmma.mma_async m64n128 (fp16: k16, int8: k32) with both operands in
 //     shared memory, fp32 / s32 accumulators in registers (64 per thread), keeping one stage's MMAs in flight while the
 //     next one is issued (wgmma.wait_group 1).  Every accumulator sums its K steps in ascending order;
-//   * two CTAs per SM (97 KB of shared memory each), so one CTA's epilogue overlaps the other's MMAs;
-//   * the epilogue works on the accumulator fragment in registers (thread = rows lane/4 and lane/4 + 8 of its warp's
-//     16 rows, columns 8j + 2(lane%4) + {0,1}): bias, fp16 rounding, activation, the row / column-block maps of
-//     GemmEpilogue, and the fused SwiGLU (a 64-column group [32 y | 32 gate] lies in one thread's columns).
+//   * two CTAs per SM (105 KB of shared memory each), so one CTA's epilogue overlaps the other's MMAs;
+//   * the epilogue computes on the accumulator fragment in registers (thread = rows lane/4 and lane/4 + 8 of its warp's
+//     16 rows, columns 8j + 2(lane%4) + {0,1}): bias, fp16 rounding, activation and the fused SwiGLU (a 64-column
+//     group [32 y | 32 gate] lies in one thread's columns); it stores through a 1 KB buffer per warp, 16 rows x 32
+//     columns at a time, in 16-byte row segments placed by the row / column-block maps of GemmEpilogue (store_block).
+//
+// Measured alone on an H100 80GB HBM3 (700 W), the shapes with large outputs reach 22-32 % of their HBM floor (hac CRF
+// head 2.77 ms against 0.72 ms, strided conv 1.09 against 0.24, sup CRF head 5.69 against 1.81).  The rest of their time
+// has not been broken down; every column tile still re-reads its CTA's A row block from L2.
 //
 // A rows may overlap (lda < K): the strided convolutions run as GEMMs over the channels-last, zero-padded stem output
 // (reference: bonito/nn.py:235-241, Conv1d k19 s6).  TMA zero-fills the rows / columns of a partial tile.
@@ -28,10 +34,56 @@ namespace {
 
 constexpr int BM = 128, BN = 128, KB = 128;          // KB: bytes of K per stage and row (one 128-byte swizzle row)
 constexpr int STAGES = 3;
+// column tiles per CTA at most.  Runs of 2 were faster alone than runs of all the tiles of a row block on every large
+// shape of the benchmarked workloads (H100 80GB HBM3, 700 W: hac CRF head 2.76 against 2.87 ms, sup fc2 1.04 against
+// 1.31 ms, sup CRF head 6.33 against 6.69 ms), and than runs of 1 or 4 on most of them.
+constexpr int MAX_RUN = 2;
 constexpr int CONSUMERS = 256, THREADS = CONSUMERS + 32;   // two consumer warpgroups + one producer warp
 constexpr uint32_t OP_BYTES = BM * KB;               // one operand slice: 16 KB
 constexpr uint32_t STAGE_BYTES = 2 * OP_BYTES;
-constexpr uint32_t SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 64;   // alignment slack + ring + 2 x STAGES mbarriers
+constexpr uint32_t EPI_BYTES = 16 * 32 * 2;          // a consumer warp's epilogue buffer: 16 rows x 32 fp16 columns
+// alignment slack + ring + 2 x STAGES mbarriers + the epilogue buffers.  Two CTAs fit on an SM (2 x (105 KB + 1 KB
+// reserved) of 228 KB); 16 KB of buffers (64 columns per warp) would leave one.
+constexpr uint32_t SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 64 + (CONSUMERS / 32) * EPI_BYTES;
+
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+// Writes a 16-row x 32-column block of the warp's results to output columns c0 .. c0 + 31 (those below n_out) of its
+// rows; orow[h]: output row of row lane/4 + 8h (-1: not written).  v[2 jj + h] is the lane's accumulator-fragment pair
+// (row lane/4 + 8h, columns 8 jj + 2(lane%4), +1).  The pairs pass through the warp's buffer `buf` (64-byte rows, 16-byte
+// chunk c of row r at chunk c ^ (r/2 % 4), so that neither stmatrix nor the read-back has bank conflicts) and come back
+// as one 16-byte chunk per lane: each store instruction writes 8 rows x 64 contiguous bytes, whole 32-byte sectors,
+// where a store of the fragment itself writes 8 rows x 16 bytes.  A column block (cb_width, a multiple of 32) never
+// splits the 32 columns.
+__device__ __forceinline__ void store_block(const uint32_t (&v)[8], uint32_t buf, int lane, const long long (&orow)[2], int c0,
+                                            int n_out, __half* C, long long ldc, const GemmEpilogue& ep) {
+    __syncwarp();   // every lane has read the previous block out of the buffer
+    {
+        const int q = lane >> 3, row = 8 * (q & 1) + (lane & 7), sw = (row >> 1) & 3;   // matrix q: (jj = 2k + q/2, h = q%2)
+#pragma unroll
+        for (int k = 0; k < 2; ++k)
+            stmatrix_x4(buf + row * 64 + 16 * ((2 * k + (q >> 1)) ^ sw), v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
+    }
+    __syncwarp();
+    const int c = lane & 3, col = c0 + 8 * c;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = 8 * h + (lane >> 2);
+        const uint4 d = ld_shared_v4(buf + row * 64 + 16 * (c ^ ((row >> 1) & 3)));
+        if (orow[h] < 0 || col >= n_out) continue;
+        long long drow = orow[h];
+        int dcol = col;
+        if (ep.cb_width > 0) {   // column-block remap
+            const int cb = col / ep.cb_width;
+            drow += (long long)cb * ep.cb_rows;
+            dcol = col - cb * ep.cb_width;
+        }
+        *reinterpret_cast<uint4*>(C + drow * ldc + dcol) = d;
+    }
+}
 
 template <bool I8>
 __global__ void __launch_bounds__(THREADS, 2)
@@ -42,9 +94,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;   // the 128-byte swizzle repeats every 1024 bytes
     const uint32_t bar_full = base + STAGES * STAGE_BYTES, bar_empty = bar_full + 8 * STAGES;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int m0 = blockIdx.x * BM;
+    const int nruns = (N + BN * tiles_per_cta - 1) / (BN * tiles_per_cta);
+    const int m0 = (int)(blockIdx.x / nruns) * BM;
     const int ntiles = (N + BN - 1) / BN;
-    const int nt0 = blockIdx.y * tiles_per_cta, nt1 = min(ntiles, nt0 + tiles_per_cta);
+    const int nt0 = (int)(blockIdx.x % nruns) * tiles_per_cta, nt1 = min(ntiles, nt0 + tiles_per_cta);
     const int ktiles = (K_bytes + KB - 1) / KB;
 
     if (tid == 0) {
@@ -75,6 +128,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
     }
 
     const int wg = warp >> 2, wq = warp & 3;
+    const uint32_t stage = bar_full + 64 + (uint32_t)warp * EPI_BYTES;
+    const int cq = 2 * (lane & 3);
+    long long orow[2];   // output rows of the lane's two rows (the same for every column tile)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int gm = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+        orow[h] = gm < M ? map_row(ep.map, gm) : -1;
+    }
     using Acc = typename std::conditional<I8, int, float>::type;
     Acc acc[64];
     int it = 0;
@@ -105,65 +166,68 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_consta
         wg_fence_regs(acc);
         if (lane == 0) mbar_arrive(bar_empty + 8 * ((it - 1) % STAGES));
 
-        const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2), cq = 2 * (lane & 3);
+        // 32-column blocks of the tile (SwiGLU: one per 64-column group, 32 outputs), each rounded into fp16 pairs
+        // v[2 jj + h] = (row lane/4 + 8h, columns 8 jj + cq, +1 of the block) and written by store_block
         if (!I8 && ep.act == B200_ACT_SWIGLU) {
             // 64-column group G of the tile: y = columns 8j' + cq + e, gate = 32 + the same; output column (n0 + 64G) / 2 + ...
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int gm = r0 + 8 * h;
-                if (gm >= M) continue;
-                const long long orow = map_row(ep.map, gm);
-                if (orow < 0) continue;
+            for (int G = 0; G < 2; ++G) {
+                const int c0 = (n0 + 64 * G) / 2;
+                if (c0 >= N / 2) continue;
+                uint32_t v[8];
 #pragma unroll
-                for (int G = 0; G < 2; ++G) {
-                    if (n0 + 64 * G >= N) continue;
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int jy = 8 * G + jj, jg = jy + 4;
 #pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        const int jy = 8 * G + jj, jg = jy + 4;
+                    for (int h = 0; h < 2; ++h) {
                         const float y0 = round_f16((float)acc[jy * 4 + h * 2]), y1 = round_f16((float)acc[jy * 4 + h * 2 + 1]);
                         const float g0 = round_f16((float)acc[jg * 4 + h * 2]), g1 = round_f16((float)acc[jg * 4 + h * 2 + 1]);
-                        const int oc = (n0 + 64 * G) / 2 + 8 * jj + cq;
-                        *reinterpret_cast<__half2*>(C + orow * ldc + oc) =
-                            __floats2half2_rn(g0 * y0 * rcp_approx(1.0f + __expf(-g0)), g1 * y1 * rcp_approx(1.0f + __expf(-g1)));
+                        v[2 * jj + h] = pack_half2(g0 * y0 * rcp_approx(1.0f + __expf(-g0)), g1 * y1 * rcp_approx(1.0f + __expf(-g1)));
                     }
                 }
+                store_block(v, stage, lane, orow, c0, N / 2, C, ldc, ep);
             }
             continue;
         }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int gm = r0 + 8 * h;
-            if (gm >= M) continue;
-            const long long orow = map_row(ep.map, gm);
-            if (orow < 0) continue;
+        for (int p = 0; p < 4; ++p) {
+            const int c0 = n0 + 32 * p;
+            if (c0 >= N) continue;
+            uint32_t v[8];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
+            for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * p + jj;
                 const int gn = n0 + 8 * j + cq;   // N % 8 == 0: the pair (gn, gn + 1) is in range together
-                if (gn >= N) continue;
-                float v0, v1;
+                const bool in = gn < N;           // pairs past N are computed from zeros and never stored
+                float s0 = 0.f, s1 = 0.f, b0 = 0.f, b1 = 0.f;
+                if (in && ep.bias) {
+                    b0 = __half2float(ep.bias[gn]);
+                    b1 = __half2float(ep.bias[gn + 1]);
+                }
                 if constexpr (I8) {
-                    const float b0 = ep.bias ? __half2float(ep.bias[gn]) : 0.f, b1 = ep.bias ? __half2float(ep.bias[gn + 1]) : 0.f;
-                    v0 = fmaf((float)acc[j * 4 + h * 2], col_scale[gn], b0);
-                    v1 = fmaf((float)acc[j * 4 + h * 2 + 1], col_scale[gn + 1], b1);
-                } else {
-                    v0 = acc[j * 4 + h * 2];
-                    v1 = acc[j * 4 + h * 2 + 1];
-                    if (ep.bias) {
-                        v0 += __half2float(ep.bias[gn]);
-                        v1 += __half2float(ep.bias[gn + 1]);
+                    if (in) {
+                        s0 = col_scale[gn];
+                        s1 = col_scale[gn + 1];
                     }
                 }
-                v0 = apply_act_f16(v0, ep.act, ep.lo, ep.hi);
-                v1 = apply_act_f16(v1, ep.act, ep.lo, ep.hi);
-                long long drow = orow;
-                int dcol = gn;
-                if (ep.cb_width > 0) {   // column-block remap (cb_width is even: a pair never straddles two blocks)
-                    const int cb = gn / ep.cb_width;
-                    drow += (long long)cb * ep.cb_rows;
-                    dcol = gn - cb * ep.cb_width;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float v0, v1;
+                    if constexpr (I8) {
+                        v0 = fmaf((float)acc[j * 4 + h * 2], s0, b0);
+                        v1 = fmaf((float)acc[j * 4 + h * 2 + 1], s1, b1);
+                    } else {
+                        v0 = acc[j * 4 + h * 2];
+                        v1 = acc[j * 4 + h * 2 + 1];
+                        if (ep.bias) {
+                            v0 += b0;
+                            v1 += b1;
+                        }
+                    }
+                    v[2 * jj + h] = pack_half2(apply_act_f16(v0, ep.act, ep.lo, ep.hi), apply_act_f16(v1, ep.act, ep.lo, ep.hi));
                 }
-                *reinterpret_cast<__half2*>(C + drow * ldc + dcol) = __floats2half2_rn(v0, v1);
             }
+            store_block(v, stage, lane, orow, c0, N, C, ldc, ep);
         }
     }
 }
@@ -209,12 +273,12 @@ int launch(const void* A, long long lda_bytes, const void* B, const float* col_s
     if (rc) return rc;
     rc = make_tma(&tb, B, I8, K_bytes / es, N, K_bytes);
     if (rc) return rc;
-    // a CTA sweeps all column tiles of its row block unless that leaves fewer than ~4 waves of CTAs (small M): then the
-    // column tiles are split into runs over blockIdx.y
+    // runs of MAX_RUN column tiles, shorter when that leaves fewer than ~4 waves of CTAs (small M); CTA b takes run
+    // b % runs of row block b / runs
     const int mblocks = (M + BM - 1) / BM, ntiles = (N + BN - 1) / BN;
-    int per = ntiles;
+    int per = ntiles < MAX_RUN ? ntiles : MAX_RUN;
     while (per > 1 && (long long)mblocks * ((ntiles + per - 1) / per) < 8LL * sms) per = (per + 1) / 2;
-    dim3 grid(mblocks, (ntiles + per - 1) / per);
+    dim3 grid(mblocks * ((ntiles + per - 1) / per));
     gemm_wgmma_kernel<I8><<<grid, THREADS, SMEM_BYTES, stream>>>(ta, tb, col_scale, C, ldc, M, N, K_bytes, per, ep);
     B200_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -222,11 +286,8 @@ int launch(const void* A, long long lda_bytes, const void* B, const float* col_s
 
 }  // namespace
 
-// max_ctas is accepted for the ABI and not needed here: the kernel is not persistent, a CTA leaves once its row block's
-// column tiles are done and the block scheduler hands the SMs to whatever else is queued.  For the hac input projection
-// (12 column tiles per CTA) that is about 0.28 ms on average: 7.0 ms alone on an H100 80GB HBM3 (700 W) for 6664 CTAs,
-// 2 x 132 resident at a time.  scripts/step_timeline.py shows no steady-state recurrent launch of the two-batch hac step
-// starting later after its input projection than with the previous one-tile-per-CTA kernel (both within 0.01 ms).
+// max_ctas is accepted for the ABI and not needed here: the kernel is not persistent, a CTA leaves once its run of
+// column tiles is done and the block scheduler hands the SMs to whatever else is queued.
 int launch_gemm_tc(const __half* A, long long lda, const __half* B, __half* C, long long ldc, int M, int N, int K,
                    const GemmEpilogue& ep, int max_ctas, cudaStream_t stream) {
     (void)max_ctas;

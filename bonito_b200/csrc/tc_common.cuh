@@ -103,6 +103,20 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int 
         "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(bar)
         : "memory");
 }
+// ---- shared-memory staging ------------------------------------------------------------------------
+// four 8x8 fp16 matrices to shared memory: lane i gives the address of row i%8 of matrix i/8 (16 bytes), register q holds
+// lane l's pair (row l/4, columns 2(l%4), +1) of matrix q -- the mma accumulator-fragment layout
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+                 "r"(r3)
+                 : "memory");
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];\n" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 // make generic-proxy writes (st.shared / st.shared::cluster) visible to the async proxy (wgmma / bulk-copy reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;\n" ::: "memory"); }
