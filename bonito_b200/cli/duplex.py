@@ -6,11 +6,13 @@ while a pool of `--threads` host threads builds the consensus of the previous ba
 
 Output: FASTQ, SAM text or BAM (BGZF-compressed on the GPU), chosen by the extension stdout is redirected to; CRAM is
 refused.
-Input: SAM text (`.sam`, what `basecaller` writes when redirected to a .sam file) or FASTQ (`.fastq` / `.fq`), chosen by
-the extension.  For each read id the first record that is neither secondary (0x100) nor supplementary (0x800) is used,
-SEQ and QUAL as stored (reverse-strand records included, as pysam's query_sequence gives them).  BAM / CRAM input and
-`--reference` (minimap2) are refused: htslib and mappy are not bundled.  `--alignment-threads` and `--mm2-preset` only
-matter with `--reference` and are accepted for compatibility.
+Input: SAM text (`.sam`), BAM (`.bam`, what `basecaller` writes when redirected to a .bam file, or any BGZF-compressed
+BAM such as htslib writes; inflated on the GPU by bonito_b200.bam) or FASTQ (`.fastq` / `.fq`), chosen by the
+extension.  For each read id the first record that is neither secondary (0x100) nor supplementary (0x800) is used, SEQ
+and QUAL as stored (reverse-strand records included, as pysam's query_sequence gives them).  A `.bam` that is empty or
+lacks the BGZF EOF marker is refused before any GPU work.  CRAM input and `--reference` (minimap2) are refused: htslib
+and mappy are not bundled.  `--alignment-threads` and `--mm2-preset` only matter with `--reference` and are accepted
+for compatibility.
 """
 
 import os
@@ -22,7 +24,7 @@ from time import perf_counter
 
 import numpy as np
 
-from bonito_b200 import duplex, native
+from bonito_b200 import bam, duplex, native
 from bonito_b200.io import DuplexBamWriter, DuplexWriter, biofmt
 from bonito_b200.multiprocessing import thread_iter
 
@@ -36,15 +38,15 @@ def _fail(msg):
 
 
 def read_format(path):
-    """"sam" / "fastq" from the extension; BAM / CRAM and anything else are refused."""
+    """"sam" / "bam" / "fastq" from the extension; CRAM and anything else are refused."""
     ext = path.lower().rsplit(".", 1)[-1] if "." in os.path.basename(path) else ""
-    if ext in ("bam", "cram"):
-        raise ValueError(f"{ext.upper()} input needs htslib, which this build does not bundle; convert to .sam or .fastq")
-    if ext == "sam":
-        return "sam"
+    if ext == "cram":
+        raise ValueError("CRAM input needs htslib, which this build does not bundle; convert to .sam or .fastq")
+    if ext in ("sam", "bam"):
+        return ext
     if ext in ("fastq", "fq"):
         return "fastq"
-    raise ValueError(f"cannot tell the format of {path}: expected a .sam, .fastq or .fq file")
+    raise ValueError(f"cannot tell the format of {path}: expected a .sam, .bam, .fastq or .fq file")
 
 
 def read_pairs(path, header=True):
@@ -84,8 +86,10 @@ def _fastq_records(fh):
 
 def read_records(path, wanted=None):
     """{read id: (sequence, qualities as uint8 Q values, or None for a QUAL of '*')} of the first primary record of each
-    id (restricted to `wanted` ids when given)."""
+    id (restricted to `wanted` ids when given).  BAM is inflated on the GPU."""
     fmt = read_format(path)
+    if fmt == "bam":
+        return bam.read_records(path, wanted)
     reads = {}
     with open(path) as fh:
         for read_id, seq, qual in (_sam_records(fh) if fmt == "sam" else _fastq_records(fh)):
@@ -152,7 +156,8 @@ def main(args):
     if args.reference:
         _fail("--reference needs minimap2 (mappy), which this build does not bundle")
     try:
-        read_format(args.in_bam)
+        if read_format(args.in_bam) == "bam":
+            bam.check_bgzf_file(args.in_bam)
     except ValueError as err:
         _fail(str(err))
     fmt = biofmt(aligned=False)
@@ -161,10 +166,13 @@ def main(args):
     sys.stderr.write(f"> outputting {fmt.aligned} {fmt.name}\n")
 
     pairs = read_pairs(args.duplex_pairs_file, header=not args.no_header)
-    reads = read_records(args.in_bam, wanted={rid for pair in pairs for rid in pair})
     try:
         native.require()
     except native.NativeError as err:
+        _fail(str(err))
+    try:
+        reads = read_records(args.in_bam, wanted={rid for pair in pairs for rid in pair})
+    except ValueError as err:
         _fail(str(err))
 
     counts = {}

@@ -1,4 +1,5 @@
-// BGZF compression (SAM specification section 4.1) for BAM output: one CTA per member of 65280 input bytes.
+// BGZF compression (SAM specification section 4.1) for BAM output: one CTA per member of 65280 input bytes; and BGZF
+// decompression for BAM input: one warp per member (inflate_member, further down).
 //
 // Per member, in one CTA (the member staged in shared memory):
 //   1. CRC32: a table CRC per thread over a contiguous slice, the slices combined by GF(2) shifts.
@@ -41,36 +42,65 @@ constexpr int COPY_THREADS = 256, SCAN_THREADS = 1024;
 constexpr int N_LIT = 286, N_DIST = 30, N_CL = 19;
 constexpr int SEL = 0x8000, IS_MATCH = 0x4000;  // per-position code word after the parse: selected, match (else literal)
 
-__constant__ uint8_t kClOrder[N_CL] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+// the order of the code-length code's lengths in a dynamic block header (RFC 1951 section 3.2.7)
+__host__ __device__ __forceinline__ int cl_order(int i) {
+    constexpr uint8_t order[N_CL] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+    return order[i];
+}
 
 using Sort = cub::BlockRadixSort<uint32_t, MEMBER_THREADS, ITEMS, uint16_t>;
 
-// length 3..258 -> literal/length symbol - 257, extra bits, extra value (RFC 1951 section 3.2.5)
+// The DEFLATE length and distance codes (RFC 1951 section 3.2.5), shared by the compressor and the inflater.
+// literal/length symbol - 257 -> base length, extra bits
+__host__ __device__ __forceinline__ void length_base(int idx, int& base, int& nbits) {
+    if (idx == 28) {
+        base = MAX_MATCH, nbits = 0;
+    } else if (idx < 8) {
+        base = 3 + idx, nbits = 0;
+    } else {
+        nbits = idx / 4 - 1;
+        base = 3 + ((4 + (idx & 3)) << nbits);
+    }
+}
+
+// distance symbol -> base distance, extra bits
+__host__ __device__ __forceinline__ void dist_base(int code, int& base, int& nbits) {
+    if (code < 4) {
+        base = 1 + code, nbits = 0;
+    } else {
+        nbits = code / 2 - 1;
+        base = 1 + ((2 + (code & 1)) << nbits);
+    }
+}
+
+// length 3..258 -> literal/length symbol - 257, extra bits, extra value
 __device__ __forceinline__ void length_code(int len, int& idx, int& nbits, int& extra) {
     const int v = len - 3;
     if (len == MAX_MATCH) {
-        idx = 28, nbits = 0, extra = 0;
+        idx = 28;
     } else if (v < 8) {
-        idx = v, nbits = 0, extra = 0;
+        idx = v;
     } else {
         const int lg = 31 - __clz(v);
         idx = 4 * (lg - 1) + ((v >> (lg - 2)) & 3);
-        nbits = idx / 4 - 1;
-        extra = v - ((4 + (idx & 3)) << nbits);
     }
+    int base;
+    length_base(idx, base, nbits);
+    extra = len - base;
 }
 
 // distance 1..32768 -> distance symbol, extra bits, extra value
 __device__ __forceinline__ void dist_code(int dist, int& code, int& nbits, int& extra) {
     const int v = dist - 1;
     if (v < 4) {
-        code = v, nbits = 0, extra = 0;
+        code = v;
     } else {
         const int lg = 31 - __clz(v);
         code = 2 * lg + ((v >> (lg - 1)) & 1);
-        nbits = code / 2 - 1;
-        extra = v - ((2 + (code & 1)) << nbits);
     }
+    int base;
+    dist_base(code, base, nbits);
+    extra = dist - base;
 }
 
 // a * b modulo the CRC polynomial, both reflected (the top bit is x^0)
@@ -89,6 +119,35 @@ __device__ uint32_t crc_shift_op(uint32_t bytes, const uint32_t* x2n) {
     for (int k = 3; bytes; bytes >>= 1, ++k)
         if (bytes & 1) p = crc_multmod(x2n[k], p);
     return p;
+}
+
+// The CRC32 of n bytes from `parts` slices taken in parallel: crc_table_entry() and crc_powers() fill the tables once,
+// crc_part() gives slice `part`'s contribution, and crc_finish() turns the XOR of every part into the CRC32.
+__device__ __forceinline__ uint32_t crc_table_entry(uint32_t c) {
+    for (int k = 0; k < 8; ++k) c = (c & 1) ? (c >> 1) ^ CRC_POLY : c >> 1;
+    return c;
+}
+
+// x2n[k] = x^(2^k), k < 32 (one thread)
+__device__ void crc_powers(uint32_t* x2n) {
+    uint32_t x = 1u << 30;  // x^1
+    for (int k = 0; k < 32; ++k) {
+        x2n[k] = x;
+        x = crc_multmod(x, x);
+    }
+}
+
+// the slice's CRC register from zero, then shifted over the bytes after it
+__device__ uint32_t crc_part(const uint8_t* buf, int n, int part, int parts, const uint32_t* table, const uint32_t* x2n) {
+    const int per = (n + parts - 1) / parts;
+    const int lo = min(n, part * per), hi = min(n, lo + per);
+    uint32_t c = 0;
+    for (int i = lo; i < hi; ++i) c = table[(c ^ buf[i]) & 0xff] ^ (c >> 8);
+    return crc_multmod(crc_shift_op((uint32_t)(n - hi), x2n), c);
+}
+
+__device__ __forceinline__ uint32_t crc_finish(uint32_t parts_xor, int n, const uint32_t* x2n) {
+    return parts_xor ^ crc_multmod(crc_shift_op((uint32_t)n, x2n), 0xffffffffu) ^ 0xffffffffu;
 }
 
 // ORs bits, LSB first, into 32-bit shared-memory words from an arbitrary bit offset
@@ -270,32 +329,16 @@ __global__ void __launch_bounds__(MEMBER_THREADS, 1)
     for (int i = tid; i < N_LIT; i += MEMBER_THREADS) s.lit_freq[i] = i == 256;  // one end-of-block symbol
     for (int i = tid; i < N_DIST; i += MEMBER_THREADS) s.dist_freq[i] = 0;
     uint32_t* crc_table = chunk_hash;  // free until phase 2
-    if (tid < 256) {
-        uint32_t c = tid;
-        for (int k = 0; k < 8; ++k) c = (c & 1) ? (c >> 1) ^ CRC_POLY : c >> 1;
-        crc_table[tid] = c;
-    }
-    if (tid == 0) {
-        uint32_t x = 1u << 30;  // x^1
-        for (int k = 0; k < 32; ++k) {
-            s.x2n[k] = x;
-            x = crc_multmod(x, x);
-        }
-    }
+    if (tid < 256) crc_table[tid] = crc_table_entry(tid);
+    if (tid == 0) crc_powers(s.x2n);
     __syncthreads();
-    {
-        const int per = (n + MEMBER_THREADS - 1) / MEMBER_THREADS;
-        const int lo = min(n, tid * per), hi = min(n, lo + per);
-        uint32_t c = 0;  // the slice's CRC register from zero, then shifted over the bytes after it
-        for (int i = lo; i < hi; ++i) c = crc_table[(c ^ buf[i]) & 0xff] ^ (c >> 8);
-        s.crc_part[tid] = crc_multmod(crc_shift_op((uint32_t)(n - hi), s.x2n), c);
-    }
+    s.crc_part[tid] = crc_part(buf, n, tid, MEMBER_THREADS, crc_table, s.x2n);
     __syncthreads();
     if (warp == 0) {
         uint32_t c = 0;
         for (int i = lane; i < MEMBER_THREADS; i += 32) c ^= s.crc_part[i];
         for (int o = 16; o; o >>= 1) c ^= __shfl_xor_sync(0xffffffffu, c, o);
-        if (lane == 0) s.crc_part[0] = c ^ crc_multmod(crc_shift_op((uint32_t)n, s.x2n), 0xffffffffu) ^ 0xffffffffu;
+        if (lane == 0) s.crc_part[0] = crc_finish(c, n, s.x2n);
     }
     __syncthreads();
     const uint32_t crc = s.crc_part[0];
@@ -443,7 +486,7 @@ __global__ void __launch_bounds__(MEMBER_THREADS, 1)
         huffman_lengths(s.cl_freq, s.cl_sorted, used, 7, s.cl_len, N_CL, s.huff_scratch[0]);
         canonical_codes(s.cl_len, N_CL, s.cl_code);
         int hclen = N_CL;
-        while (hclen > 4 && !s.cl_len[kClOrder[hclen - 1]]) --hclen;
+        while (hclen > 4 && !s.cl_len[cl_order(hclen - 1)]) --hclen;
         int bits = 3 + 5 + 5 + 4 + 3 * hclen;
         for (int i = 0; i < m; ++i) {
             const int sym = s.rle_sym[i];
@@ -497,7 +540,7 @@ __global__ void __launch_bounds__(MEMBER_THREADS, 1)
             bw.put(s.hlit - 257, 5);
             bw.put(s.hdist - 1, 5);
             bw.put(s.hclen - 4, 4);
-            for (int i = 0; i < s.hclen; ++i) bw.put(s.cl_len[kClOrder[i]], 3);
+            for (int i = 0; i < s.hclen; ++i) bw.put(s.cl_len[cl_order(i)], 3);
             for (int i = 0; i < s.n_rle; ++i) {
                 const int sym = s.rle_sym[i];
                 bw.put(s.cl_code[sym], s.cl_len[sym]);
@@ -595,6 +638,318 @@ __global__ void __launch_bounds__(COPY_THREADS) bgzf_copy_kernel(const uint8_t* 
     for (int i = threadIdx.x; i < size; i += COPY_THREADS) to[i] = from[i];
 }
 
+// ------------------------------------------------------------------------------------------------ inflate
+// RFC 1951 inflation of one BGZF member, written once for the device (a warp, all lanes in lockstep) and the host (one
+// "lane"): every lane reads the same bits and decodes the same symbols, so control flow stays uniform; lane 0 writes the
+// literals, and the lanes share the Huffman table fills, match copies and stored-block copies.  A member's window is its
+// own output (BGZF members share no history).  Every input read is bounded by in_len (bits peeked past it read as
+// zeros; consuming them is an error), every output write by out_len.
+constexpr int LIT_BITS = 10, DIST_BITS = 8;  // primary lookup bits; longer codes are decoded canonically
+constexpr int N_LIT_SYMS = 288, N_DIST_SYMS = 32, MAX_BITS = 15;
+
+struct InflateScratch {
+    uint16_t lit_lut[1 << LIT_BITS];    // (symbol << 4) | length, 0 when the code is longer than LIT_BITS or unused
+    uint16_t dist_lut[1 << DIST_BITS];  // the same; first the code-length code's table
+    uint16_t lit_sym[N_LIT_SYMS];       // symbols in canonical order
+    uint16_t dist_sym[N_DIST_SYMS];
+    uint16_t lit_count[MAX_BITS + 1];   // codes of each length
+    uint16_t dist_count[MAX_BITS + 1];
+    uint16_t first[MAX_BITS + 1];       // while a table is built: the first code of each length,
+    uint16_t start[MAX_BITS + 1];       // the canonical index of that code,
+    uint16_t fill[MAX_BITS + 1];        // and the next free canonical index
+    uint8_t lens[N_LIT_SYMS + N_DIST_SYMS];
+};
+
+__host__ __device__ __forceinline__ void lanes_sync(int lanes) {
+#ifdef __CUDA_ARCH__
+    __syncwarp(lanes >= 32 ? 0xffffffffu : (1u << lanes) - 1);
+#endif
+}
+
+__host__ __device__ __forceinline__ uint8_t load_in(const uint8_t* p) {
+#ifdef __CUDA_ARCH__
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+
+__host__ __device__ __forceinline__ uint32_t reverse_bits(uint32_t v, int n) {
+#ifdef __CUDA_ARCH__
+    return __brev(v) >> (32 - n);
+#else
+    uint32_t r = 0;
+    for (int i = 0; i < n; ++i, v >>= 1) r = r << 1 | (v & 1);
+    return r;
+#endif
+}
+
+struct Huff {
+    uint16_t* lut;
+    uint16_t* sym;
+    uint16_t* count;
+    int bits;
+};
+
+// Canonical code of lens[0..n): count[], sym[] and the primary table.  Returns 0 for a complete code or no code at all,
+// 1 for the one incomplete code DEFLATE allows (a single code of length 1, when allow_single), -1 otherwise.  The counts
+// and canonical offsets live in the warp's shared scratch, written by lane 0; the lanes then fill the table from the
+// canonical order, each its own symbols.
+__host__ __device__ int huff_build(const uint8_t* lens, int n, const Huff& h, bool allow_single, InflateScratch& s,
+                                   int lane, int lanes) {
+    lanes_sync(lanes);  // every lane is done with the table this one replaces
+    if (lane == 0) {
+        for (int l = 0; l <= MAX_BITS; ++l) h.count[l] = 0;
+        for (int i = 0; i < n; ++i) ++h.count[lens[i]];
+    }
+    lanes_sync(lanes);
+    const int used = n - h.count[0];
+    int left = 1;
+    for (int l = 1; l <= MAX_BITS; ++l) {
+        left = (left << 1) - h.count[l];
+        if (left < 0) return -1;  // over-subscribed
+    }
+    int status = 0;
+    if (left > 0 && used > 0) {
+        if (!(allow_single && used == 1 && h.count[1] == 1)) return -1;
+        status = 1;
+    }
+    if (lane == 0) {
+        int code = 0, pos = 0;
+        for (int l = 1; l <= MAX_BITS; ++l) {
+            code = (code + (l > 1 ? h.count[l - 1] : 0)) << 1;
+            s.first[l] = (uint16_t)code;
+            s.start[l] = s.fill[l] = (uint16_t)pos;
+            pos += h.count[l];
+        }
+        for (int i = 0; i < n; ++i)
+            if (lens[i]) h.sym[s.fill[lens[i]]++] = (uint16_t)i;
+    }
+    const int size = 1 << h.bits;
+    for (int k = lane; k < size; k += lanes) h.lut[k] = 0;
+    lanes_sync(lanes);
+    for (int i = lane; i < used; i += lanes) {
+        const int sym = h.sym[i], l = lens[sym];
+        if (l > h.bits) break;  // canonical order: every later code is as long
+        const int code = s.first[l] + i - s.start[l];
+        const uint16_t e = (uint16_t)(sym << 4 | l);
+        for (int k = (int)reverse_bits(code, l); k < size; k += 1 << l) h.lut[k] = e;
+    }
+    lanes_sync(lanes);
+    return status;
+}
+
+struct BitReader {
+    const uint8_t* in;
+    int len, pos, cnt;  // pos: next byte to load (runs past len when zeros are peeked)
+    uint64_t buf;
+    __host__ __device__ void refill() {
+        while (cnt <= 56) {
+            buf |= (uint64_t)(pos < len ? load_in(in + pos) : 0) << cnt;
+            ++pos;
+            cnt += 8;
+        }
+    }
+    __host__ __device__ __forceinline__ uint32_t take(int n) {
+        const uint32_t v = (uint32_t)(buf & ((1ull << n) - 1));
+        buf >>= n;
+        cnt -= n;
+        return v;
+    }
+    __host__ __device__ __forceinline__ bool overrun() const { return (int64_t)pos * 8 - cnt > (int64_t)len * 8; }
+    // more than the 8 bytes the buffer can hold peeked past the end: the bits consumed have already passed it
+    __host__ __device__ __forceinline__ bool far_overrun() const { return pos > len + 8; }
+};
+
+// one symbol, with at least MAX_BITS bits in the buffer; -1 for bits that match no code
+__host__ __device__ __forceinline__ int huff_decode(BitReader& br, const Huff& h) {
+    const uint16_t e = h.lut[br.buf & ((1u << h.bits) - 1)];
+    if (e) {
+        br.take(e & 15);
+        return e >> 4;
+    }
+    int code = 0, first = 0, index = 0;  // canonical decode, one bit at a time
+    for (int l = 1; l <= MAX_BITS; ++l) {
+        code |= (int)((br.buf >> (l - 1)) & 1);
+        const int c = h.count[l];
+        if (code - c < first) {
+            br.take(l);
+            return h.sym[index + code - first];
+        }
+        index += c;
+        first = (first + c) << 1;
+        code <<= 1;
+    }
+    return -1;
+}
+
+// The dynamic block header: code lengths into lens[], then both tables.
+__host__ __device__ int read_dynamic(BitReader& br, InflateScratch& s, const Huff& lit, const Huff& dist, int lane,
+                                     int lanes) {
+    br.refill();
+    const int hlit = (int)br.take(5) + 257, hdist = (int)br.take(5) + 1, hclen = (int)br.take(4) + 4;
+    if (hlit > 286 || hdist > 30) return B200_INFLATE_CODE_LENGTHS;
+    lanes_sync(lanes);  // every lane is past the previous block's lengths
+    if (lane == 0)
+        for (int i = 0; i < N_CL; ++i) s.lens[i] = 0;
+    br.refill();  // 3 * 19 bits: two refills
+    for (int i = 0; i < hclen; ++i) {
+        if (i == 16) br.refill();
+        const uint8_t v = (uint8_t)br.take(3);
+        if (lane == 0) s.lens[cl_order(i)] = v;
+    }
+    const Huff cl = {s.dist_lut, s.dist_sym, s.dist_count, 7};
+    if (huff_build(s.lens, N_CL, cl, false, s, lane, lanes) != 0) return B200_INFLATE_CODE_LENGTHS;
+    const int total = hlit + hdist;
+    for (int i = 0; i < total;) {
+        br.refill();
+        if (br.far_overrun()) return B200_INFLATE_TRUNCATED;
+        const int sym = huff_decode(br, cl);
+        if (sym < 0) return B200_INFLATE_CODE_LENGTHS;
+        if (sym < 16) {
+            if (lane == 0) s.lens[i] = (uint8_t)sym;
+            ++i;
+            continue;
+        }
+        int len = 0, rep;
+        if (sym == 16) {
+            if (i == 0) return B200_INFLATE_REPEAT;
+            lanes_sync(lanes);
+            len = s.lens[i - 1];
+            rep = 3 + (int)br.take(2);
+        } else if (sym == 17) {
+            rep = 3 + (int)br.take(3);
+        } else {
+            rep = 11 + (int)br.take(7);
+        }
+        if (i + rep > total) return B200_INFLATE_REPEAT;
+        if (lane == 0)
+            for (int k = 0; k < rep; ++k) s.lens[i + k] = (uint8_t)len;
+        i += rep;
+    }
+    lanes_sync(lanes);
+    if (s.lens[256] == 0) return B200_INFLATE_CODE_LENGTHS;  // no end-of-block code
+    if (huff_build(s.lens, hlit, lit, true, s, lane, lanes) < 0) return B200_INFLATE_CODE_LENGTHS;
+    if (huff_build(s.lens + hlit, hdist, dist, true, s, lane, lanes) < 0) return B200_INFLATE_CODE_LENGTHS;
+    return B200_INFLATE_OK;
+}
+
+__host__ __device__ int read_fixed(InflateScratch& s, const Huff& lit, const Huff& dist, int lane, int lanes) {
+    lanes_sync(lanes);
+    if (lane == 0) {
+        for (int i = 0; i < N_LIT_SYMS; ++i) s.lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
+        for (int i = 0; i < N_DIST_SYMS; ++i) s.lens[N_LIT_SYMS + i] = 5;
+    }
+    lanes_sync(lanes);
+    const int l = huff_build(s.lens, N_LIT_SYMS, lit, false, s, lane, lanes);
+    const int d = huff_build(s.lens + N_LIT_SYMS, N_DIST_SYMS, dist, false, s, lane, lanes);
+    return l || d ? B200_INFLATE_CODE_LENGTHS : B200_INFLATE_OK;
+}
+
+// Inflates the raw DEFLATE stream in[0..in_len) into exactly out[0..out_len); a B200_INFLATE_* status.  Every lane of
+// the group [0, lanes) calls it with the same arguments and gets the same status.
+__host__ __device__ int inflate_member(const uint8_t* in, int in_len, uint8_t* out, int out_len, InflateScratch& s,
+                                       int lane, int lanes) {
+    const Huff lit = {s.lit_lut, s.lit_sym, s.lit_count, LIT_BITS};
+    const Huff dist = {s.dist_lut, s.dist_sym, s.dist_count, DIST_BITS};
+    BitReader br = {in, in_len, 0, 0, 0};
+    int op = 0;
+    for (bool last = false; !last;) {
+        br.refill();
+        if (br.overrun()) return B200_INFLATE_TRUNCATED;
+        last = br.take(1);
+        const int type = (int)br.take(2);
+        if (type == 0) {  // stored: to the byte boundary, LEN, NLEN, LEN bytes
+            br.take(br.cnt & 7);
+            int bp = br.pos - br.cnt / 8;
+            if (bp + 4 > in_len) return B200_INFLATE_TRUNCATED;
+            const int n = load_in(in + bp) | load_in(in + bp + 1) << 8;
+            const int nn = load_in(in + bp + 2) | load_in(in + bp + 3) << 8;
+            if (n != (~nn & 0xffff)) return B200_INFLATE_STORED_LENGTH;
+            bp += 4;
+            if (n > in_len - bp) return B200_INFLATE_TRUNCATED;
+            if (n > out_len - op) return B200_INFLATE_OVERFLOW;
+            for (int i = lane; i < n; i += lanes) out[op + i] = load_in(in + bp + i);
+            op += n;
+            br.pos = bp + n, br.cnt = 0, br.buf = 0;
+            continue;
+        }
+        if (type == 3) return B200_INFLATE_BLOCK_TYPE;
+        const int st = type == 1 ? read_fixed(s, lit, dist, lane, lanes) : read_dynamic(br, s, lit, dist, lane, lanes);
+        if (st) return st;
+        for (;;) {
+            br.refill();  // >= 57 bits: a length code, its extra bits, a distance code and its extra bits
+            if (br.far_overrun()) return B200_INFLATE_TRUNCATED;
+            const int sym = huff_decode(br, lit);
+            if (sym < 256) {
+                if (sym < 0) return B200_INFLATE_SYMBOL;
+                if (op >= out_len) return B200_INFLATE_OVERFLOW;
+                if (lane == 0) out[op] = (uint8_t)sym;
+                ++op;
+                continue;
+            }
+            if (sym == 256) break;
+            if (sym > 285) return B200_INFLATE_SYMBOL;
+            int len, nb;
+            length_base(sym - 257, len, nb);
+            len += (int)br.take(nb);
+            const int dsym = huff_decode(br, dist);
+            if (dsym < 0 || dsym >= 30) return B200_INFLATE_SYMBOL;
+            int d;
+            dist_base(dsym, d, nb);
+            d += (int)br.take(nb);
+            if (d > op) return B200_INFLATE_DISTANCE;
+            if (len > out_len - op) return B200_INFLATE_OVERFLOW;
+            lanes_sync(lanes);  // the bytes before op are written
+            // the match repeats out[op - d, op) with period d, so every byte reads from before op
+            const uint8_t* from = out + op - d;
+            const int step = lanes % d;
+            for (int i = lane, j = lane % d; i < len; i += lanes) {
+                out[op + i] = from[j];
+                j += step;
+                if (j >= d) j -= d;
+            }
+            op += len;
+        }
+        if (br.overrun()) return B200_INFLATE_TRUNCATED;
+    }
+    lanes_sync(lanes);
+    return op == out_len ? B200_INFLATE_OK : B200_INFLATE_SHORT;
+}
+
+constexpr int INFLATE_WARPS = 4;
+
+// one warp per member; meta[m] = raw DEFLATE start in `in`, its length, output offset, ISIZE, expected CRC32
+__global__ void __launch_bounds__(INFLATE_WARPS * 32)
+    bgzf_inflate_kernel(const uint8_t* __restrict__ in, int64_t in_bytes, const int64_t* __restrict__ meta, int n_members,
+                        uint8_t* __restrict__ out, int64_t out_bytes, int32_t* __restrict__ status) {
+    __shared__ InflateScratch scratch[INFLATE_WARPS];
+    __shared__ uint32_t crc_table[256], x2n[32];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int i = tid; i < 256; i += INFLATE_WARPS * 32) crc_table[i] = crc_table_entry(i);
+    if (tid == 0) crc_powers(x2n);
+    __syncthreads();
+    const int64_t m = (int64_t)blockIdx.x * INFLATE_WARPS + warp;
+    if (m >= n_members) return;
+    const int64_t* mm = meta + 5 * m;
+    const int64_t in_start = mm[0], in_len = mm[1], out_start = mm[2], isize = mm[3];
+    const uint32_t crc = (uint32_t)mm[4];
+    int st;
+    if (in_start < 0 || in_len < 0 || in_len > in_bytes - in_start || isize < 0 || isize > SLOT || out_start < 0 ||
+        isize > out_bytes - out_start) {
+        st = B200_INFLATE_BOUNDS;
+    } else {
+        uint8_t* dst = out + out_start;
+        st = inflate_member(in + in_start, (int)in_len, dst, (int)isize, scratch[warp], lane, 32);
+        if (st == B200_INFLATE_OK) {
+            uint32_t c = crc_part(dst, (int)isize, lane, 32, crc_table, x2n);
+            for (int o = 16; o; o >>= 1) c ^= __shfl_xor_sync(0xffffffffu, c, o);
+            if (crc_finish(c, (int)isize, x2n) != crc) st = B200_INFLATE_CRC;
+        }
+    }
+    if (lane == 0) status[m] = st;
+}
+
 struct Layout {
     size_t sizes, slots, prev, dist, total;
 };
@@ -638,6 +993,18 @@ int b200_bgzf_compress(const uint8_t* in, int64_t in_bytes, uint8_t* out, int64_
         in, in_bytes, ws + l.slots, (int*)(ws + l.sizes), (uint16_t*)(ws + l.prev), (uint16_t*)(ws + l.dist));
     bgzf_scan_kernel<<<1, SCAN_THREADS, 0, st>>>((const int*)(ws + l.sizes), members, out_offsets);
     bgzf_copy_kernel<<<(unsigned)members, COPY_THREADS, 0, st>>>(ws + l.slots, out_offsets, out);
+    B200_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int b200_bgzf_decompress(const uint8_t* in, int64_t in_bytes, const int64_t* meta, int n_members, uint8_t* out,
+                         int64_t out_bytes, int32_t* status, void* stream) {
+    B200_REQUIRE(n_members >= 0 && in_bytes >= 0 && out_bytes >= 0, "bgzf_decompress: negative size");
+    if (n_members == 0) return 0;
+    B200_REQUIRE(meta && status && (in || in_bytes == 0) && (out || out_bytes == 0), "bgzf_decompress: null pointer argument");
+    const unsigned blocks = (unsigned)((n_members + INFLATE_WARPS - 1) / INFLATE_WARPS);
+    bgzf_inflate_kernel<<<blocks, INFLATE_WARPS * 32, 0, (cudaStream_t)stream>>>(in, in_bytes, meta, n_members, out, out_bytes,
+                                                                               status);
     B200_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -123,10 +123,17 @@ SIGNATURES = {
                                c_void_p]),
     "b200_bgzf_workspace_bytes": (c_size_t, [c_longlong]),
     "b200_bgzf_compress": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "b200_bgzf_decompress": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_longlong, c_void_p, c_void_p]),
 }
 
 BGZF_MEMBER_INPUT = 65280   # B200_BGZF_MEMBER_INPUT
 BGZF_MEMBER_MAX = 65536     # output bytes per member at most
+# B200_INFLATE_* status codes of b200_bgzf_decompress
+INFLATE_STATUS = {1: "block type 3", 2: "stored block LEN is not the complement of NLEN",
+                  3: "invalid Huffman code lengths", 4: "invalid code-length repeat",
+                  5: "invalid literal/length or distance code", 6: "distance reaches before the member's first byte",
+                  7: "output longer than ISIZE", 8: "output shorter than ISIZE", 9: "DEFLATE data ends before the final block",
+                  10: "CRC32 mismatch", 11: "member outside the launch's buffers"}
 
 
 class NativeError(RuntimeError):
@@ -854,3 +861,21 @@ def bgzf_compress(inp, out, out_offsets, workspace, stream=None):
                                     _stream(stream))
     _check(rc, "b200_bgzf_compress")
     return out_offsets
+
+
+def bgzf_decompress(inp, meta, out, status, stream=None):
+    """Inflate BGZF members (see b200_bgzf_decompress): inp CUDA uint8 (the members' raw DEFLATE data), meta CUDA int64
+    [n, 5] (raw start, raw length, output offset, ISIZE, CRC32 per member), out CUDA uint8, status CUDA int32 [n]
+    (INFLATE_STATUS codes, 0 = inflated and CRC32 verified)."""
+    lib = require()
+    what = "bgzf_decompress"
+    _dev(inp, torch.uint8, "inp", what)
+    _dev(out, torch.uint8, "out", what)
+    n = meta.shape[0] if isinstance(meta, torch.Tensor) else 0
+    _dev(meta, torch.int64, "meta", what, (n, 5))
+    _dev(status, torch.int32, "status", what, (n,))
+    with torch.cuda.device(out.device):
+        rc = lib.b200_bgzf_decompress(_ptr(inp), inp.numel(), _ptr(meta), n, _ptr(out), out.numel(), _ptr(status),
+                                      _stream(stream))
+    _check(rc, "b200_bgzf_decompress")
+    return status

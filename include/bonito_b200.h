@@ -23,6 +23,8 @@
  *   b200_ctc_beam_search      fast_ctc_decode.beam_search             bonito/ctc/model.py:39-46, ctc/basecall.py:43-61
  *   b200_bgzf_compress        htslib bgzf_write, reached through      bonito/io.py:400-503
  *                             pysam AlignmentFile(..., 'wb') (BAM output)
+ *   b200_bgzf_decompress      htslib bgzf_read, reached through       bonito/cli/duplex.py:45-105
+ *                             pysam in bonito/cli/duplex.py (BAM input of `duplex`)
  *
  * Conventions (SURVEY.md section 8b): every function returns 0 on success and a negative value on
  * failure, with a message available from b200_last_error().  All pointers are raw DEVICE pointers
@@ -501,6 +503,32 @@ int b200_map_align(const void* query, const void* target, const void* chain, con
 size_t b200_bgzf_workspace_bytes(int64_t in_bytes);
 int b200_bgzf_compress(const uint8_t* in, int64_t in_bytes, uint8_t* out, int64_t* out_offsets, void* workspace,
                        size_t workspace_bytes, void* stream);
+
+/*
+ * ---- BGZF decompression for BAM input (RFC 1951 inflation of each member's raw DEFLATE data) ----
+ * meta: DEVICE int64 [n_members][5] = start of the member's raw DEFLATE data in `in` (DEVICE bytes [in_bytes]), its
+ * length, the member's output offset in `out` (DEVICE bytes [out_bytes]), its ISIZE (<= 65536) and its expected CRC32.
+ * Each member is inflated into out[offset, offset + ISIZE) by one warp; any valid DEFLATE stream is accepted (stored,
+ * fixed and dynamic Huffman blocks, any number of blocks, distances up to 32768).  status: DEVICE int32 [n_members]
+ * receives one B200_INFLATE_* code per member.  A malformed member gets a nonzero status and never faults: reads stay
+ * within its raw data and writes within its output slot, and its neighbours are decoded as if it were absent.
+ */
+#define B200_INFLATE_OK 0
+#define B200_INFLATE_BLOCK_TYPE 1     /* a block of type 3 */
+#define B200_INFLATE_STORED_LENGTH 2  /* a stored block whose LEN is not the complement of NLEN */
+#define B200_INFLATE_CODE_LENGTHS 3   /* HLIT > 286 or HDIST > 30; an over-subscribed or incomplete code (DEFLATE allows one
+                                         length-1 code alone); no end-of-block code; bits that match no code-length code */
+#define B200_INFLATE_REPEAT 4         /* code-length repeat 16 with no previous length, or a repeat past HLIT + HDIST */
+#define B200_INFLATE_SYMBOL 5         /* literal/length symbol 286 or 287, distance code 30 or 31, or bits that match no
+                                         literal/length or distance code */
+#define B200_INFLATE_DISTANCE 6       /* a distance reaching before the member's first output byte */
+#define B200_INFLATE_OVERFLOW 7       /* output past ISIZE */
+#define B200_INFLATE_SHORT 8          /* fewer than ISIZE bytes at the end of the final block */
+#define B200_INFLATE_TRUNCATED 9      /* more bits consumed than the raw data holds */
+#define B200_INFLATE_CRC 10           /* the CRC32 of the output differs from the expected one */
+#define B200_INFLATE_BOUNDS 11        /* the member's meta row reaches outside in / out, or ISIZE > 65536 */
+int b200_bgzf_decompress(const uint8_t* in, int64_t in_bytes, const int64_t* meta, int n_members, uint8_t* out,
+                         int64_t out_bytes, int32_t* status, void* stream);
 
 #ifdef __cplusplus
 }
