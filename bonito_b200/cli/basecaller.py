@@ -1,6 +1,8 @@
 """
 `bonito_b200 basecaller <model_directory> <reads_directory>` -- the flag surface of the reference's
 `bonito basecaller` (`bonito/cli/basecaller.py:168-199`) over the native engine.
+Reads come from `*.pod5` files (bonito_b200.pod5: VBZ signal decompressed on the GPU, no pod5 package needed; SAM and BAM
+output carry the run info's @RG lines) or from `*.npy` files of picoampere samples (bonito_b200.reader).
 Output is FASTQ, or SAM text with the `mv:B:c` move table when stdout is redirected to a `.sam` file, or BAM with the same
 records when it is redirected to a `.bam` file, BGZF-compressed on the GPU (the reference's `biofmt` rule,
 bonito/io.py:35-54); CRAM is refused.  `--reference <fasta>` maps the calls on the GPU (bonito_b200.aligner, this
@@ -50,6 +52,9 @@ def main(args):
         sys.stderr.write("> reading %s\n" % reader.fmt)
     except FileNotFoundError:
         sys.stderr.write("> error: no suitable files found in %s\n" % args.reads_directory)
+        exit(1)
+    except ValueError as err:                   # a malformed POD5 file
+        sys.stderr.write(f"> error: {err}\n")
         exit(1)
     fmt = biofmt(aligned=args.reference is not None)
     if fmt.mode not in ("wfq", "w", "wb"):
@@ -117,7 +122,10 @@ def main(args):
                        chunksize=params["chunksize"], overlap=params["overlap"], **decode_args)
     if aligner:
         results = align_map(aligner, results, n_thread=args.alignment_threads)
-    writer_args = dict(min_qscore=args.min_qscore, group_key=os.path.basename(os.path.normpath(args.model_directory)),
+    group_key = os.path.basename(os.path.normpath(args.model_directory))
+    # the @RG lines of the POD5 run info, keyed like the records' RG:Z tags (bonito/cli/basecaller.py:86-95); none for .npy
+    groups = reader.get_read_groups(args.reads_directory, group_key, recursive=args.recursive) if fmt.name != "fastq" else []
+    writer_args = dict(min_qscore=args.min_qscore, group_key=group_key, groups=groups,
                        contigs=aligner.contigs if aligner else None)
     if args.save_ctc:
         writer = CtcWriter(results, aligner, mode=fmt.mode, min_qscore=args.min_qscore,

@@ -124,6 +124,9 @@ SIGNATURES = {
     "b200_bgzf_workspace_bytes": (c_size_t, [c_longlong]),
     "b200_bgzf_compress": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "b200_bgzf_decompress": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_longlong, c_void_p, c_void_p]),
+    "b200_zstd_decompress": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_longlong, c_void_p, c_void_p,
+                                     c_void_p]),
+    "b200_svb16_decode": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_void_p, c_longlong, c_void_p, c_void_p]),
 }
 
 BGZF_MEMBER_INPUT = 65280   # B200_BGZF_MEMBER_INPUT
@@ -878,4 +881,52 @@ def bgzf_decompress(inp, meta, out, status, stream=None):
         rc = lib.b200_bgzf_decompress(_ptr(inp), inp.numel(), _ptr(meta), n, _ptr(out), out.numel(), _ptr(status),
                                       _stream(stream))
     _check(rc, "b200_bgzf_decompress")
+    return status
+
+
+# ------------------------------------------------------------------------------------------------ zstd / svb16 (zstd.cu)
+# B200_ZSTD_* status codes of b200_zstd_decompress
+ZSTD_STATUS = {0: "ok", 1: "not a zstd frame", 2: "reserved frame header bit, dictionary ID or window too large",
+               3: "reserved block type or block too large", 4: "invalid literals section size or type",
+               5: "invalid Huffman weights or literal stream", 6: "invalid FSE table or accuracy log",
+               7: "invalid sequence count or bit stream", 8: "offset before the frame's first byte",
+               9: "output past capacity", 10: "content size mismatch", 11: "truncated input", 12: "checksum mismatch",
+               13: "stream outside the launch's buffers"}
+# B200_SVB16_* status codes of b200_svb16_decode
+SVB16_STATUS = {0: "ok", 1: "svb16 length is not keys + data", 2: "row outside the launch's buffers"}
+
+
+def zstd_decompress(inp, meta, out, out_len, status, stream=None):
+    """Decompress zstd streams (see b200_zstd_decompress): inp CUDA uint8, meta CUDA int64 [n, 4] (input offset, input
+    length, output offset, output capacity per stream), out CUDA uint8, out_len CUDA int64 [n] (bytes produced), status
+    CUDA int32 [n] (ZSTD_STATUS codes, 0 = decoded)."""
+    lib = require()
+    what = "zstd_decompress"
+    _dev(inp, torch.uint8, "inp", what)
+    _dev(out, torch.uint8, "out", what)
+    n = meta.shape[0] if isinstance(meta, torch.Tensor) else 0
+    _dev(meta, torch.int64, "meta", what, (n, 4))
+    _dev(out_len, torch.int64, "out_len", what, (n,))
+    _dev(status, torch.int32, "status", what, (n,))
+    with torch.cuda.device(out.device):
+        rc = lib.b200_zstd_decompress(_ptr(inp), inp.numel(), _ptr(meta), n, _ptr(out), out.numel(), _ptr(out_len),
+                                      _ptr(status), _stream(stream))
+    _check(rc, "b200_zstd_decompress")
+    return status
+
+
+def svb16_decode(inp, meta, out, status, stream=None):
+    """Decode svb16 rows into int16 samples (see b200_svb16_decode): inp CUDA uint8, meta CUDA int64 [n, 4] (svb16
+    offset, svb16 length, sample count, sample offset per row), out CUDA int16, status CUDA int32 [n] (SVB16_STATUS)."""
+    lib = require()
+    what = "svb16_decode"
+    _dev(inp, torch.uint8, "inp", what)
+    _dev(out, torch.int16, "out", what)
+    n = meta.shape[0] if isinstance(meta, torch.Tensor) else 0
+    _dev(meta, torch.int64, "meta", what, (n, 4))
+    _dev(status, torch.int32, "status", what, (n,))
+    with torch.cuda.device(out.device):
+        rc = lib.b200_svb16_decode(_ptr(inp), inp.numel(), _ptr(meta), n, _ptr(out), out.numel(), _ptr(status),
+                                   _stream(stream))
+    _check(rc, "b200_svb16_decode")
     return status

@@ -1,11 +1,14 @@
 """
 Read ingestion for `bonito_b200 basecaller`.
 
-The reference picks a pod5 or fast5 reader by globbing the reads directory (`bonito/reader.py:23-48`);
-both need third-party libraries (pod5, ont_fast5_api) that are optional here.  Supported inputs:
-  * `*.pod5`  through the `pod5` package when it is importable (signal in pA = scale * (raw + offset));
+The reference picks a pod5 or fast5 reader by globbing the reads directory (`bonito/reader.py:23-48`).  Supported
+inputs:
+  * `*.pod5`  read by bonito_b200.pod5 without the pod5 package: the container parsed on the host, the VBZ signal rows
+              decompressed on the GPU, signal in pA = scale * (raw + offset), the reference's metadata and @RG lines;
+              reads in reads-table order, `read_ids` / `skip` matched against the read UUID strings;
   * `*.npy`   one read per file: a 1-D array of picoampere samples, read id = file stem (what the tests and the
-              synthetic benchmarks use; no third-party dependency).
+              synthetic benchmarks use); no metadata and no read groups.
+fast5 input is not supported.
 Trimming and normalisation follow `bonito/reader.py:122-166` (trim of the leading stall, pA standardisation or
 quantile scaling).
 """
@@ -63,6 +66,10 @@ class Read:
         self.shift, self.scale = normalisation(pa, scaling_strategy, norm_params)
         self.trimmed_samples = trim(pa, threshold=self.scale * 2.4 + self.shift) if do_trim else 0
         self.template_start = self.trimmed_samples
+        if "sample_rate" in meta:  # POD5: positions in seconds (bonito/pod5.py:44-65)
+            self.sample_rate, self.start = meta["sample_rate"], meta["start"]
+            self.template_start = self.start + self.trimmed_samples / self.sample_rate
+            self.template_duration = meta["duration"] - self.trimmed_samples / self.sample_rate
         self.signal = ((pa[self.trimmed_samples:] - self.shift) / self.scale).astype(np.float32)
         self.scaling_strategy = (scaling_strategy or {}).get("strategy") or "quantile"
         # acquisition metadata the SAM tags carry (bonito/reader.py:59-87); .npy reads have none
@@ -122,6 +129,9 @@ def read_chunks(read, chunksize=4000, overlap=400):
 
 
 class Reader:
+    """The reads of a directory: `*.pod5` files if there are any, else `*.npy` files.  Every POD5 file's container is
+    checked here, so a malformed one is refused (ValueError naming it) before any CUDA use."""
+
     def __init__(self, directory, recursive=False):
         self.fmt = None
         for fmt in ("pod5", "npy"):
@@ -132,27 +142,36 @@ class Reader:
         if self.fmt is None:
             raise FileNotFoundError(directory)
         if self.fmt == "pod5":
-            try:
-                import pod5  # noqa: F401
-            except ImportError as err:
-                raise FileNotFoundError(f"{directory}: pod5 files found but the `pod5` package is not installed") from err
+            from bonito_b200.pod5 import Pod5File
+            for path in self._paths(directory, recursive):
+                Pod5File(path)
+
+    def _paths(self, directory, recursive):
+        pattern = f"**/*.{self.fmt}" if recursive else f"*.{self.fmt}"
+        return sorted(glob(os.path.join(directory, pattern), recursive=True))
 
     def get_reads(self, directory, recursive=False, read_ids=None, skip=False, do_trim=True, scaling_strategy=None,
-                  norm_params=None, **_ignored):
-        pattern = f"**/*.{self.fmt}" if recursive else f"*.{self.fmt}"
-        for path in sorted(glob(os.path.join(directory, pattern), recursive=True)):
-            for read_id, pa in self._signals(path):
+                  norm_params=None, device=None, **_ignored):
+        for path in self._paths(directory, recursive):
+            if self.fmt == "npy":
+                read_id = os.path.splitext(os.path.basename(path))[0]
                 if read_ids is not None and ((read_id in read_ids) == bool(skip)):
                     continue
-                yield Read(read_id, pa, filename=os.path.basename(path), do_trim=do_trim,
+                yield Read(read_id, np.load(path), filename=os.path.basename(path), do_trim=do_trim,
                            scaling_strategy=scaling_strategy, norm_params=norm_params)
+                continue
+            from bonito_b200.pod5 import Pod5File, pa_signal
+            for read_id, raw, offset, scale, meta in Pod5File(path).signals(read_ids, skip, device=device):
+                yield Read(read_id, pa_signal(raw, offset, scale), filename=os.path.basename(path), do_trim=do_trim,
+                           scaling_strategy=scaling_strategy, norm_params=norm_params, meta=meta)
 
-    def _signals(self, path):
-        if self.fmt == "npy":
-            yield os.path.splitext(os.path.basename(path))[0], np.load(path)
-            return
-        import pod5
-        with pod5.Reader(path) as reader:
-            for rec in reader.reads():
-                cal = rec.calibration
-                yield str(rec.read_id), cal.scale * (rec.signal.astype(np.float32) + cal.offset)
+    def get_read_groups(self, directory, model, recursive=False, **_ignored):
+        """The reference's @RG header lines of every POD5 file's run info (bonito/pod5.py:84-110), sorted; none for
+        `.npy` input."""
+        if self.fmt != "pod5":
+            return []
+        from bonito_b200.pod5 import Pod5File
+        groups = set()
+        for path in self._paths(directory, recursive):
+            groups |= Pod5File(path).read_groups(model)
+        return sorted(groups)

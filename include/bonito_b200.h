@@ -25,6 +25,10 @@
  *                             pysam AlignmentFile(..., 'wb') (BAM output)
  *   b200_bgzf_decompress      htslib bgzf_read, reached through       bonito/cli/duplex.py:45-105
  *                             pysam in bonito/cli/duplex.py (BAM input of `duplex`)
+ *   b200_zstd_decompress      libzstd ZSTD_decompress, reached through bonito/pod5.py:12,57
+ *                             pod5.Reader (the zstd stage of VBZ signal rows)
+ *   b200_svb16_decode         lib_pod5 decompress_signal (svb16 +      bonito/pod5.py:12,57
+ *                             delta + zigzag stage of VBZ), through pod5.Reader
  *
  * Conventions (SURVEY.md section 8b): every function returns 0 on success and a negative value on
  * failure, with a message available from b200_last_error().  All pointers are raw DEVICE pointers
@@ -529,6 +533,47 @@ int b200_bgzf_compress(const uint8_t* in, int64_t in_bytes, uint8_t* out, int64_
 #define B200_INFLATE_BOUNDS 11        /* the member's meta row reaches outside in / out, or ISIZE > 65536 */
 int b200_bgzf_decompress(const uint8_t* in, int64_t in_bytes, const int64_t* meta, int n_members, uint8_t* out,
                          int64_t out_bytes, int32_t* status, void* stream);
+
+/*
+ * ---- zstd decompression for POD5 signal input (RFC 8878; the decoder is this library's, in bonito_b200/csrc/zstd.cu) ----
+ * meta: DEVICE int64 [n][4] = a stream's offset in `in` (DEVICE bytes [in_bytes]), its length, its output offset in `out`
+ * (DEVICE bytes [out_bytes]) and its output capacity.  Each stream is decoded by one warp as ZSTD_decompress decodes it
+ * without a dictionary: one or more frames back to back, skippable frames skipped; Raw, RLE and Compressed blocks; every
+ * literals and sequences mode; the optional Frame_Content_Size (must equal the frame's output) and XXH64 checksum (must
+ * match).  out_len: DEVICE int64 [n] receives the bytes written, status: DEVICE int32 [n] one B200_ZSTD_* code per stream.
+ * A malformed stream gets a nonzero status and never faults: reads stay within its input range, writes within its output
+ * slot (which a failed stream may leave partly written, past out_len too), and its neighbours decode as if it were absent.
+ */
+#define B200_ZSTD_OK 0
+#define B200_ZSTD_MAGIC 1          /* neither a zstd frame nor a skippable frame (legacy formats included) */
+#define B200_ZSTD_FRAME_HEADER 2   /* the reserved frame header bit set, a nonzero dictionary ID, or a window above 2^31 */
+#define B200_ZSTD_BLOCK_TYPE 3     /* a block of the reserved type 3, or a compressed block larger than 128 KiB */
+#define B200_ZSTD_LITERALS 4       /* a literals section whose sizes exceed the block or 128 KiB, or Treeless with no table */
+#define B200_ZSTD_HUFFMAN 5        /* invalid Huffman weights, or a Huffman literal stream not consumed exactly */
+#define B200_ZSTD_FSE 6            /* an invalid FSE table description or accuracy log, or Repeat mode with no table */
+#define B200_ZSTD_SEQUENCES 7      /* a bad sequence count or modes byte, a bit stream not consumed exactly, or a literal
+                                      length past the block's literals */
+#define B200_ZSTD_OFFSET 8         /* a match offset before the frame's first byte or beyond its window */
+#define B200_ZSTD_OVERFLOW 9       /* output past the stream's capacity */
+#define B200_ZSTD_CONTENT_SIZE 10  /* output of a frame differs from its Frame_Content_Size */
+#define B200_ZSTD_TRUNCATED 11     /* the input ends inside a frame or a skippable frame */
+#define B200_ZSTD_CHECKSUM 12      /* the XXH64 content checksum differs */
+#define B200_ZSTD_BOUNDS 13        /* the stream's meta row reaches outside in / out */
+int b200_zstd_decompress(const uint8_t* in, int64_t in_bytes, const int64_t* meta, int n, uint8_t* out, int64_t out_bytes,
+                         int64_t* out_len, int32_t* status, void* stream);
+
+/*
+ * ---- svb16 decoding for POD5 signal input (the StreamVByte-16, delta and zigzag stages of VBZ) ----
+ * meta: DEVICE int64 [n][4] = a row's svb16 offset in `in` (DEVICE bytes [in_bytes]), its svb16 length, its sample count
+ * and its sample offset in `out` (DEVICE int16 [out_samples]).  A row holds ceil(count / 8) key bytes, LSB first (a set
+ * bit: that value takes two bytes, little-endian; else one), then the data bytes; each value is unzigzagged and the
+ * samples are its modular 16-bit prefix sum from 0.  One warp per row; status: DEVICE int32 [n] one B200_SVB16_* code.
+ */
+#define B200_SVB16_OK 0
+#define B200_SVB16_LENGTH 1  /* the svb16 length is not exactly the keys plus the data bytes they call for */
+#define B200_SVB16_BOUNDS 2  /* the row's meta row reaches outside in / out */
+int b200_svb16_decode(const uint8_t* in, int64_t in_bytes, const int64_t* meta, int n, int16_t* out, int64_t out_samples,
+                      int32_t* status, void* stream);
 
 #ifdef __cplusplus
 }
