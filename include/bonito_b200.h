@@ -553,7 +553,9 @@ int b200_bgzf_decompress(const uint8_t* in, int64_t in_bytes, const int64_t* met
 #define B200_ZSTD_FSE 6            /* an invalid FSE table description or accuracy log, or Repeat mode with no table */
 #define B200_ZSTD_SEQUENCES 7      /* a bad sequence count or modes byte, a bit stream not consumed exactly, or a literal
                                       length past the block's literals */
-#define B200_ZSTD_OFFSET 8         /* a match offset before the frame's first byte or beyond its window */
+#define B200_ZSTD_OFFSET 8         /* a match offset before the frame's first byte or beyond its window, or a repeat
+                                      offset Rep1 - 1 of 0 (libzstd decodes both: the window bound it does not check,
+                                      and the zero offset it reads as 1) */
 #define B200_ZSTD_OVERFLOW 9       /* output past the stream's capacity */
 #define B200_ZSTD_CONTENT_SIZE 10  /* output of a frame differs from its Frame_Content_Size */
 #define B200_ZSTD_TRUNCATED 11     /* the input ends inside a frame or a skippable frame */
