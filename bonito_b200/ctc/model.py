@@ -12,6 +12,8 @@ Decoding: `greedy_step` / `greedy_collapse` (host, the default) and `beam_search
 with fast_ctc_decode's beam search of width 5 (bonito/ctc/model.py:39-46).  Deviations: the default here is the greedy
 decode; the beam search returns qualities and emission frames, which the reference's has not, so `qscores=True` keeps the
 beam search where the reference switches to its Viterbi decode; there is no CPU path for the beam search.
+
+Loss: `loss` / `ctc_label_smoothing_loss` as in the reference, with the CTC loss on the GPU (`bonito_b200.ctc.loss`).
 """
 
 import numpy as np
@@ -103,6 +105,29 @@ class Model(Module):
         if return_path:
             return seq, np.flatnonzero(moves)
         return seq
+
+    def ctc_label_smoothing_loss(self, log_probs, targets, lengths, weights=None):
+        """
+        CTC loss plus label smoothing (reference: bonito/ctc/model.py:48-54).  `log_probs` is the reference layout
+        [T, N, C] on a CUDA device; the native forward's [N, T, C] output becomes it by `permute(1, 0, 2)`, which the
+        loss reads in place.  Every input length is T, the CTC loss (`bonito_b200.ctc.loss.ctc_loss`, on the GPU) has
+        reduction 'mean', and the smoothing term is -(log_probs * weights).mean() in torch's type promotion, as in the
+        reference; `weights` defaults to [0.4, 0.1 / (C - 1), ...].  Deviation: a given `weights` tensor is used as it
+        is, where the reference's `weights or ...` raises for one of more than one element.
+        Returns {'total_loss', 'loss', 'label_smooth_loss'}.
+        """
+        from bonito_b200.ctc.loss import ctc_loss
+        T, N, C = log_probs.shape
+        if weights is None:
+            weights = torch.cat([torch.tensor([0.4]), (0.1 / (C - 1)) * torch.ones(C - 1)])
+        log_probs_lengths = torch.full(size=(N,), fill_value=T, dtype=torch.int64)
+        loss = ctc_loss(log_probs.to(torch.float32), targets, log_probs_lengths, lengths, reduction="mean")
+        label_smoothing_loss = -((log_probs * weights.to(log_probs.device)).mean())
+        return {"total_loss": loss + label_smoothing_loss, "loss": loss, "label_smooth_loss": label_smoothing_loss}
+
+    def loss(self, log_probs, targets, lengths):
+        """`ctc_label_smoothing_loss` with the default weights (reference: bonito/ctc/model.py:56-57)."""
+        return self.ctc_label_smoothing_loss(log_probs, targets, lengths)
 
 
 MAX_BEAMSIZE = 32

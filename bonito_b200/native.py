@@ -109,6 +109,12 @@ SIGNATURES = {
                                         c_void_p]),
     "b200_ctc_crf_target_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_loss_max_target": (c_int, []),
+    "b200_ctc_loss_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "b200_ctc_loss_fwd": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_int, c_int, c_void_p, c_void_p, c_longlong,
+                                  c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_loss_grad": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_int, c_int, c_void_p, c_void_p, c_longlong,
+                                   c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "b200_ctc_beam_workspace_bytes": (c_size_t, [c_int, c_longlong, c_int]),
     "b200_ctc_beam_search": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_float, c_void_p, c_size_t,
                                      c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -661,6 +667,71 @@ def ctc_crf_target_grad(stay, move, lengths, semiring, g, workspace, dstay, dmov
                                           _ptr(g), _ptr(workspace), _ptr(dstay), _ptr(dmove), _stream(stream))
     _check(rc, "b200_ctc_crf_target_grad")
     return dstay, dmove
+
+
+def ctc_loss_max_target():
+    return load().b200_ctc_loss_max_target()
+
+
+def ctc_loss_workspace_bytes(n, t, max_target):
+    return load().b200_ctc_loss_workspace_bytes(int(n), int(t), int(max_target))
+
+
+def _ctc_loss_shape(log_probs, input_lengths, targets, target_off, target_lengths, what):
+    if not isinstance(log_probs, torch.Tensor) or not log_probs.is_cuda or log_probs.dtype != torch.float32 \
+            or log_probs.dim() != 3 or (log_probs.stride(2) != 1 and log_probs.shape[2] != 1):
+        raise NativeError(f"{what}: log_probs must be a CUDA fp32 [T, N, C] tensor with a contiguous class axis")
+    t, n, _ = log_probs.shape
+    _dev(input_lengths, torch.int32, "input_lengths", what, (n,))
+    _dev(target_lengths, torch.int32, "target_lengths", what, (n,))
+    _dev(target_off, torch.int64, "target_off", what, (n,))
+    _dev(targets, torch.int32, "targets", what)
+    return log_probs.shape
+
+
+def ctc_loss_fwd(log_probs, input_lengths, targets, target_off, target_lengths, max_target, blank, nll, workspace=None,
+                 stream=None):
+    """CTC negative log-likelihood (see b200_ctc_loss_fwd): log_probs CUDA fp32 [T, N, C] (any strides on T and N);
+    input_lengths / target_lengths int32 [N]; sample n's labels are targets.view(-1)[target_off[n]:][:target_lengths[n]]
+    (int32 targets, int64 target_off) -> nll [N]; `workspace` (uint8, ctc_loss_workspace_bytes bytes) keeps what
+    ctc_loss_grad needs."""
+    lib = require()
+    what = "ctc_loss_fwd"
+    t, n, c = _ctc_loss_shape(log_probs, input_lengths, targets, target_off, target_lengths, what)
+    _dev(nll, torch.float32, "nll", what, (n,))
+    if workspace is not None:
+        _dev(workspace, torch.uint8, "workspace", what)
+        need = ctc_loss_workspace_bytes(n, t, max_target)
+        if workspace.numel() < need:
+            raise NativeError(f"{what}: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(log_probs.device):
+        rc = lib.b200_ctc_loss_fwd(_ptr(log_probs), log_probs.stride(0), log_probs.stride(1), t, n, c, _ptr(input_lengths),
+                                   _ptr(targets), targets.numel(), _ptr(target_off), _ptr(target_lengths), int(max_target),
+                                   int(blank), _ptr(nll), _ptr(workspace), _stream(stream))
+    _check(rc, "b200_ctc_loss_fwd")
+    return nll
+
+
+def ctc_loss_grad(log_probs, input_lengths, targets, target_off, target_lengths, max_target, blank, g, zero_infinity,
+                  workspace, grad, stream=None):
+    """grad [T, N, C] = g[n] * dnll[n]/dlog_probs in torch's form, from the workspace of ctc_loss_fwd with the same
+    arguments (see b200_ctc_loss_grad)."""
+    lib = require()
+    what = "ctc_loss_grad"
+    t, n, c = _ctc_loss_shape(log_probs, input_lengths, targets, target_off, target_lengths, what)
+    _dev(g, torch.float32, "g", what, (n,))
+    _dev(grad, torch.float32, "grad", what, (t, n, c))
+    _dev(workspace, torch.uint8, "workspace", what)
+    need = ctc_loss_workspace_bytes(n, t, max_target)
+    if workspace.numel() < need:
+        raise NativeError(f"{what}: workspace has {workspace.numel()} bytes, {need} needed")
+    with torch.cuda.device(log_probs.device):
+        rc = lib.b200_ctc_loss_grad(_ptr(log_probs), log_probs.stride(0), log_probs.stride(1), t, n, c, _ptr(input_lengths),
+                                    _ptr(targets), targets.numel(), _ptr(target_off), _ptr(target_lengths), int(max_target),
+                                    int(blank), _ptr(g), int(bool(zero_infinity)), _ptr(workspace), _ptr(grad),
+                                    _stream(stream))
+    _check(rc, "b200_ctc_loss_grad")
+    return grad
 
 
 def ctc_beam_workspace_bytes(n_reads, total_frames, beam_width):

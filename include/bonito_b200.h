@@ -20,6 +20,8 @@
  *                             (_lb: learned blank scores, heads without blank_score, bonito/crf/model.py:150-162)
  *   b200_ctc_crf_*            koi.ctc (logZ_cu_sparse, fwd/bwd_scores_  bonito/crf/model.py:30-143
  *                             cu_sparse, logZ_cu, viterbi_alignments)
+ *   b200_ctc_loss_*           torch.nn.functional.ctc_loss behind     bonito/ctc/model.py:48-57
+ *                             Model.loss of the QuartzNet models
  *   b200_ctc_beam_search      fast_ctc_decode.beam_search             bonito/ctc/model.py:39-46, ctc/basecall.py:43-61
  *   b200_bgzf_compress        htslib bgzf_write, reached through      bonito/io.py:400-503
  *                             pysam AlignmentFile(..., 'wb') (BAM output)
@@ -437,6 +439,37 @@ int b200_ctc_crf_target_fwd(const void* stay, const void* move, const void* leng
                             void* logz, void* workspace, void* stream);
 int b200_ctc_crf_target_grad(const void* stay, const void* move, const void* lengths, int t, int n, int l, int semiring,
                              const void* g, void* workspace, void* dstay, void* dmove, void* stream);
+
+/*
+ * ---- CTC loss (reference: torch.nn.functional.ctc_loss in Model.ctc_label_smoothing_loss, bonito/ctc/model.py:48-57;
+ *      the recursions, the gradient and the work split are stated in bonito_b200/csrc/ctc_loss.cu) ----
+ * log_probs: DEVICE fp32 [t][n][c], element (t', n', c') at t' * stride_t + n' * stride_n + c' (the class axis is
+ * contiguous; stride_t and stride_n are any non-negative element strides, so a permuted [n][t][c] tensor is read in place).
+ * input_lengths, target_lengths: DEVICE int32 [n]; sample n's labels are the int32 targets[target_off[n] ..
+ * target_off[n] + target_lengths[n]) of DEVICE targets [n_targets], target_off DEVICE int64 [n] (padded [n][s] targets:
+ * target_off[n'] = n' * s).  1 <= c <= B200_CTC_LOSS_MAX_CLASSES, 0 <= blank < c, every target length <= max_target <=
+ * b200_ctc_loss_max_target(); out-of-range host arguments return -2 before anything is launched.  A sample with an input
+ * length outside 1..t, a target length outside 0..max_target, labels outside targets or a label outside [0, c) gets a NaN
+ * loss and gradient; nothing is read or written outside the arrays.
+ *   b200_ctc_loss_fwd:  nll [n] fp32, the negative log-likelihood (inf where no alignment fits).  With `workspace` (of
+ *     b200_ctc_loss_workspace_bytes(n, t, max_target) bytes: the log-domain alpha of every frame) it keeps what
+ *     b200_ctc_loss_grad needs; NULL computes the loss alone.
+ *   b200_ctc_loss_grad: grad [t][n][c] fp32 contiguous = g[n'] * dnll[n']/dlog_probs in torch's form, from the workspace of
+ *     a forward with the same arguments: (exp(lp) - exp(lcab + nll - lp)) * g for frames before the input length, exactly
+ *     0 after it; an infinite nll gives NaN on those frames, or 0 when zero_infinity is nonzero.
+ * Every output is bitwise reproducible (no atomics).
+ */
+#define B200_CTC_LOSS_MAX_TARGET 4096 /* labels per target: 2 * 4096 + 1 states */
+#define B200_CTC_LOSS_MAX_CLASSES 256
+int b200_ctc_loss_max_target(void);
+size_t b200_ctc_loss_workspace_bytes(int n, int t, int max_target);
+int b200_ctc_loss_fwd(const void* log_probs, long long stride_t, long long stride_n, int t, int n, int c,
+                      const void* input_lengths, const void* targets, long long n_targets, const void* target_off,
+                      const void* target_lengths, int max_target, int blank, void* nll, void* workspace, void* stream);
+int b200_ctc_loss_grad(const void* log_probs, long long stride_t, long long stride_n, int t, int n, int c,
+                       const void* input_lengths, const void* targets, long long n_targets, const void* target_off,
+                       const void* target_lengths, int max_target, int blank, const void* g, int zero_infinity,
+                       void* workspace, void* grad, void* stream);
 
 /*
  * ---- CTC prefix beam search (reference: fast_ctc_decode.beam_search behind bonito/ctc/model.py:39-46; that crate's output
