@@ -2,9 +2,9 @@
 from argparse import ArgumentParser, ArgumentDefaultsHelpFormatter
 
 from bonito_b200 import __version__
-from bonito_b200.cli import basecaller, duplex, evaluate
+from bonito_b200.cli import basecaller, duplex, evaluate, train
 
-modules = ["basecaller", "duplex", "evaluate"]
+modules = ["basecaller", "duplex", "evaluate", "train"]
 
 
 def main():
@@ -13,7 +13,7 @@ def main():
     subparsers = parser.add_subparsers(title="subcommands", description="valid commands", help="additional help",
                                        dest="command")
     subparsers.required = True
-    for name, mod in (("basecaller", basecaller), ("duplex", duplex), ("evaluate", evaluate)):
+    for name, mod in (("basecaller", basecaller), ("duplex", duplex), ("evaluate", evaluate), ("train", train)):
         p = subparsers.add_parser(name, parents=[mod.argparser()])
         p.set_defaults(func=mod.main)
     args = parser.parse_args()

@@ -5,7 +5,13 @@ QuartzNet CTC model package (`package = "bonito.ctc"`: dna_r9.4.1@v1 and @v2).
 the same attribute names and registration order), so a reference `weights_N.tar` loads through `match_names` unchanged,
 BatchNorm running statistics included.  On the CPU without `use_koi` the module tree runs and returns `[T, N, 5]`
 log-probs, as the reference's `forward` does.  With `use_koi` the native engine (`bonito_b200.engine_ctc.CtcPlan`) runs
-it on the GPU and returns batch-first `[N, T, 5]` fp16 log-probs; there is no eager CUDA path.
+it on the GPU and returns batch-first `[N, T, 5]` fp16 log-probs; there is no eager CUDA path.  The plan holds folded
+copies of the weights and BatchNorm statistics: it remembers the `_version` of every parameter and buffer it folded and is
+rebuilt when any of them changes (an optimizer step, a `load_state_dict`, a training forward's statistics update).
+
+Training: in train mode with grad enabled, a CUDA input runs `bonito_b200.engine_ctc.CtcTrainPlan` through one autograd
+node (`CtcTrainFunction`): batch-statistics BatchNorm, dropout, fp16 operands with fp32 accumulation, and fp32
+`[N, T, 5]` log-probs that backpropagate into every parameter on native kernels.
 
 Decoding: `greedy_step` / `greedy_collapse` (host, the default) and `beam_search`, the CTC prefix beam search on the GPU
 (`b200_ctc_beam_search`; cut, merge, tie, move and quality rules in bonito_b200/csrc/ctc_beam.cu).  The reference decodes
@@ -41,15 +47,29 @@ class Model(Module):
         self.decoder = Decoder(self.features, len(self.alphabet))
         self._native = None        # set by use_koi(): dict of basecaller settings
         self._plan = None          # built lazily, after the weights are loaded
+        self._plan_state = None    # (data_ptr, _version) of every parameter and buffer when the plan was built
+        self._train_plan = None
 
     def forward(self, x):
-        """[N, 1, L] -> log-probs: [T, N, 5] from the module tree on the CPU, [N, T, 5] fp16 from the native engine."""
+        """[N, 1, L] -> log-probs: [T, N, 5] from the module tree on the CPU, [N, T, 5] fp16 from the native engine, and
+        [N, T, 5] fp32 from the native training path (train mode, grad enabled, CUDA input)."""
         if self._native is None:
             if x.is_cuda:
                 raise RuntimeError("bonito_b200: CUDA model called without use_koi(); call model.use_koi(...) "
                                    "(load_model(..., use_koi=True)) or run the module tree on the CPU")
             return self.decoder(self.encoder(x))
+        if self.training and torch.is_grad_enabled() and x.is_cuda:
+            from bonito_b200 import native
+            from bonito_b200.engine_ctc import CtcTrainFunction, CtcTrainPlan
+            native.require()
+            if self._train_plan is None:
+                self._train_plan = CtcTrainPlan(self)
+            seed = int(torch.randint(0, 2**62, (1,)).item())
+            return CtcTrainFunction.apply(self._train_plan, seed, x, *self._train_plan.params)
         return self.native_plan(x.device if x.is_cuda else None).forward(x)
+
+    def _state(self):
+        return [(t.data_ptr(), t._version) for t in list(self.parameters()) + list(self.buffers())]
 
     def native_plan(self, device=None):
         from bonito_b200 import native
@@ -59,19 +79,21 @@ class Model(Module):
             device = next(self.parameters()).device
         if torch.device(device).type != "cuda":
             raise native.NativeError("the native path was requested (use_koi) but the model is not on a CUDA device")
-        if self._plan is None or self._plan.device != torch.device(device):
+        state = self._state()
+        if self._plan is None or self._plan.device != torch.device(device) or self._plan_state != state:
             self._plan = CtcPlan(self, device, quantize=bool((self._native or {}).get("quantize")))
+            self._plan_state = state
         return self._plan
 
     def invalidate_plan(self):
-        self._plan = None
+        self._plan = self._train_plan = None
 
     def _apply(self, fn, *args, **kwargs):
-        self._plan = None  # .half()/.to() change the tensors the plan was packed from
+        self._plan = self._train_plan = None  # .half()/.to() change the tensors the plans were packed from / refer to
         return super()._apply(fn, *args, **kwargs)
 
     def apply(self, fn):
-        self._plan = None
+        self._plan = self._train_plan = None
         return super().apply(fn)
 
     def load_state_dict(self, *args, **kwargs):
@@ -81,7 +103,7 @@ class Model(Module):
     def use_koi(self, **kwargs):
         """Arm the native engine (the hook `_load_model` calls)."""
         self._native = dict(kwargs)
-        self._plan = None
+        self._plan = self._train_plan = None
 
     def decode(self, x, beamsize=1, threshold=1e-3, qscores=False, return_path=False):
         """

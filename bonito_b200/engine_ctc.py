@@ -46,59 +46,74 @@ def _fold(conv, bn):
     return w * s[:, None, None], b
 
 
+def _walk(model):
+    """Validate the `Encoder` / `Block` / `TCSConv1d` / `Decoder` tree against the shape rules of the native kernels; one
+    dict per block with its (TCSConv1d, BatchNorm1d) pairs, residual modules and shapes, and the head Conv1d."""
+    from bonito_b200.ctc.model import Block, TCSConv1d
+    blocks = list(model.encoder.encoder)
+    if not blocks or not all(isinstance(b, Block) for b in blocks):
+        raise UnsupportedModel("native CTC path needs an Encoder of Blocks")
+    out = []
+    for i, blk in enumerate(blocks):
+        act = blk.activation[0]
+        name = getattr(type(act), "name", None)
+        if name not in _ACTS:
+            raise UnsupportedModel(f"activation {act!r} has no native kernel (relu, swish)")
+        mods = [m for m in blk.conv if isinstance(m, (TCSConv1d, torch.nn.BatchNorm1d))]
+        pairs = list(zip(mods[0::2], mods[1::2]))
+        if len(mods) % 2 or not all(isinstance(t, TCSConv1d) and isinstance(b, torch.nn.BatchNorm1d) for t, b in pairs):
+            raise UnsupportedModel("a Block must be repeat x [TCSConv1d, BatchNorm1d]")
+        separable = pairs[0][0].separable
+        convs = [t.depthwise if separable else t.conv for t, _ in pairs]
+        k = convs[0].kernel_size[0]
+        for c in convs + ([t.pointwise for t, _ in pairs] if separable else []):
+            if c.dilation[0] != 1:
+                raise UnsupportedModel("dilated convolutions have no native kernel")
+            if c.padding[0] != c.kernel_size[0] // 2:
+                raise UnsupportedModel("convolutions must use padding k // 2")
+        stride = convs[0].stride[0]
+        if i == 0:
+            if separable or convs[0].in_channels != 1 or len(pairs) != 1 or blk.use_res:
+                raise UnsupportedModel("the first block must be a 1-channel dense convolution with repeat 1")
+            if stride > 8 or k > 33 or k % 2 == 0 or convs[0].out_channels > 512:
+                raise UnsupportedModel(f"first convolution 1 -> {convs[0].out_channels} k{k} s{stride} has no native kernel")
+        elif stride != 1:
+            raise UnsupportedModel("only the first block may be strided")
+        elif k % 2 == 0:        # padding k // 2 would give T + 1 frames: every block here keeps T
+            raise UnsupportedModel(f"an even kernel size (k{k}) has no native path")
+        if not separable and blk.use_res:
+            raise UnsupportedModel("a residual connection on a non-separable block has no native path")
+        if not separable and len(pairs) > 1:
+            raise UnsupportedModel("a non-separable block with repeat > 1 has no native path")
+        cin = pairs[0][0].depthwise.in_channels if separable else convs[0].in_channels
+        cout = pairs[-1][1].num_features
+        if separable:
+            for t, _ in pairs:
+                if not depthwise_supported(t.depthwise.in_channels, k):
+                    raise UnsupportedModel(f"depthwise convolution C={t.depthwise.in_channels} k{k} has no native kernel")
+        out.append(dict(block=blk, pairs=pairs, separable=separable, residual=bool(blk.use_res), act=_ACTS[name], k=k,
+                        stride=stride, cin=cin, cout=cout))
+    head = model.decoder.layers[0]
+    if head.out_channels != 5 or head.kernel_size[0] != 1 or head.in_channels % 8:
+        raise UnsupportedModel("the decoder must be Conv1d(features -> 5, k1) with features % 8 == 0")
+    return out, head
+
+
 class CtcPlan:
     supports_slots = False
 
     def __init__(self, model, device, quantize=False):
-        from bonito_b200.ctc.model import Block, TCSConv1d
         if quantize:
             raise UnsupportedModel("int8 (--quantize) has no native path for the QuartzNet CTC models")
         self.device = dev = torch.device(device)
-        blocks = list(model.encoder.encoder)
-        if not blocks or not all(isinstance(b, Block) for b in blocks):
-            raise UnsupportedModel("native CTC path needs an Encoder of Blocks")
+        walked, head = _walk(model)
         self.blocks = []
-        for i, blk in enumerate(blocks):
-            act = blk.activation[0]
-            name = getattr(type(act), "name", None)
-            if name not in _ACTS:
-                raise UnsupportedModel(f"activation {act!r} has no native kernel (relu, swish)")
-            mods = [m for m in blk.conv if isinstance(m, (TCSConv1d, torch.nn.BatchNorm1d))]
-            pairs = list(zip(mods[0::2], mods[1::2]))
-            if len(mods) % 2 or not all(isinstance(t, TCSConv1d) and isinstance(b, torch.nn.BatchNorm1d) for t, b in pairs):
-                raise UnsupportedModel("a Block must be repeat x [TCSConv1d, BatchNorm1d]")
-            separable = pairs[0][0].separable
-            convs = [t.depthwise if separable else t.conv for t, _ in pairs]
-            k = convs[0].kernel_size[0]
-            for c in convs + ([t.pointwise for t, _ in pairs] if separable else []):
-                if c.dilation[0] != 1:
-                    raise UnsupportedModel("dilated convolutions have no native kernel")
-                if c.padding[0] != c.kernel_size[0] // 2:
-                    raise UnsupportedModel("convolutions must use padding k // 2")
-            stride = convs[0].stride[0]
-            if i == 0:
-                if separable or convs[0].in_channels != 1 or len(pairs) != 1 or blk.use_res:
-                    raise UnsupportedModel("the first block must be a 1-channel dense convolution with repeat 1")
-                if stride > 8 or k > 33 or k % 2 == 0 or convs[0].out_channels > 512:
-                    raise UnsupportedModel(f"first convolution 1 -> {convs[0].out_channels} k{k} s{stride} has no native kernel")
-            elif stride != 1:
-                raise UnsupportedModel("only the first block may be strided")
-            elif k % 2 == 0:        # padding k // 2 would give T + 1 frames: every block here keeps T
-                raise UnsupportedModel(f"an even kernel size (k{k}) has no native path")
-            if not separable and blk.use_res:
-                raise UnsupportedModel("a residual connection on a non-separable block has no native path")
-            if not separable and len(pairs) > 1:
-                raise UnsupportedModel("a non-separable block with repeat > 1 has no native path")
-            act_code = _ACTS[name]
-            cin = pairs[0][0].depthwise.in_channels if separable else convs[0].in_channels
-            cout = pairs[-1][1].num_features
-            b = dict(separable=separable, residual=bool(blk.use_res), act=act_code, k=k, stride=stride, cin=cin, cout=cout,
-                     reps=[])
-            if separable:
+        for i, wb in enumerate(walked):
+            blk, pairs, k, cin, cout = wb["block"], wb["pairs"], wb["k"], wb["cin"], wb["cout"]
+            b = dict(separable=wb["separable"], residual=wb["residual"], act=wb["act"], k=k, stride=wb["stride"], cin=cin,
+                     cout=cout, reps=[])
+            if wb["separable"]:
                 for r, (t, bn) in enumerate(pairs):
-                    cdw = t.depthwise.in_channels
-                    if not depthwise_supported(cdw, k):
-                        raise UnsupportedModel(f"depthwise convolution C={cdw} k{k} has no native kernel")
                     w, bias = _fold(t.pointwise, bn)
                     w = w[:, :, 0]
                     if r == len(pairs) - 1 and blk.use_res:
@@ -107,10 +122,10 @@ class CtcPlan:
                         w, bias = torch.cat([w, wr[:, :, 0]], dim=1), bias + br
                     if w.shape[1] % 8 or cout % 8:
                         raise UnsupportedModel("pointwise widths must be multiples of 8")
-                    b["reps"].append(dict(cdw=cdw, wd=_dev16(t.depthwise.weight.detach(), dev), w=_dev16(w, dev),
-                                          b=_dev16(bias, dev)))
+                    b["reps"].append(dict(cdw=t.depthwise.in_channels, wd=_dev16(t.depthwise.weight.detach(), dev),
+                                          w=_dev16(w, dev), b=_dev16(bias, dev)))
             else:
-                w, bias = _fold(convs[0], pairs[0][1])
+                w, bias = _fold(pairs[0][0].conv, pairs[0][1])
                 if i == 0:
                     b["w"] = _dev16(w, dev)
                 else:
@@ -119,10 +134,7 @@ class CtcPlan:
                     b["w"] = _dev16(w.permute(0, 2, 1).reshape(cout, -1), dev)      # [Cout][tap * Cin + cin]
                 b["b"] = _dev16(bias, dev)
             self.blocks.append(b)
-        head = model.decoder.layers[0]
         self.features = head.in_channels
-        if head.out_channels != 5 or head.kernel_size[0] != 1 or self.features % 8:
-            raise UnsupportedModel("the decoder must be Conv1d(features -> 5, k1) with features % 8 == 0")
         self.wh = _dev16(head.weight.detach()[:, :, 0], dev)
         self.bh = _dev16(None if head.bias is None else head.bias.detach(), dev)
         self.stride = self.blocks[0]["stride"]
@@ -244,3 +256,306 @@ class CtcPlan:
                         gemm(dw, dw_ld, rep["w"], rep["b"], bufs["h"], b["cout"], M, M, M, 0, b["act"])
                     cur, cur_ld = bufs["h"], b["cout"]
         return bufs, N, T
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# Training (train mode, grad enabled): batch-statistics BatchNorm, dropout, and the backward pass
+# ------------------------------------------------------------------------------------------------------------------------
+class CtcTrainPlan:
+    """
+    Training forward and backward of the module tree on the GPU, with torch's train-mode semantics under fp16 autocast.
+
+    Forward, per convolution + BatchNorm: the pre-BatchNorm convolution runs on the inference kernels with no bias and no
+    activation (`b200_conv_first_fwd_ex`, `b200_depthwise_conv_fwd`, `b200_gemm_fwd_ex`; v2's k15 dense conv over a
+    zero-haloed buffer), then `b200_bn_stats` (batch mean and biased variance over the N*T frames, eps and momentum of the
+    module, running statistics updated in place) and `b200_bn_act_fwd` (BatchNorm, the residual branch's BatchNorm in a
+    residual block, activation, dropout with the block's p).  The residual branch keeps its own statistics, so a residual
+    block runs the last pointwise conv and the 1x1 residual conv as two GEMMs.  Operands are fp16 with fp32 accumulation;
+    the fp32 master weights are cast to fp16 once per forward.  The head returns fp32 log-probs [N, T, 5].
+
+    Dropout: element (frame, channel) of dropout layer u is kept by a counter-based hash of (seed, u, index); the seed is
+    drawn from torch's CPU generator on every forward (Model.forward), so torch.manual_seed makes a run reproducible.
+    The keep bits are saved for the backward pass.
+
+    Backward: `b200_ctc_head_bwd`; per BatchNorm `b200_bn_act_bwd` (the activation input recomputed from the saved
+    pre-BatchNorm tensors); weight gradients by `b200_wgrad_gemm` (pointwise, residual, dense; the k15 conv in one call
+    over the haloed buffer), `b200_depthwise_wgrad` and `b200_conv_first_wgrad`; input gradients by the forward kernels:
+    `b200_gemm_fwd_ex` with the weight transposed (the k15 conv over a haloed dz with the taps reversed) and
+    `b200_depthwise_conv_fwd` with the taps reversed.  The two gradients into a residual block's input are summed inside
+    the next `b200_bn_act_bwd` (depthwise path first).  Every kernel is deterministic, so two identical steps give
+    bitwise-equal gradients.
+
+    Everything saved lives in the object `forward` returns (held by the autograd graph), never in plan buffers, so any
+    number of forwards may precede their backwards.
+    """
+
+    def __init__(self, model):
+        self.walked, self.head = _walk(model)
+        self.params = []
+        for wb in self.walked:
+            blk = wb["block"]
+            drops = [m.p for m in list(blk.conv) + list(blk.activation) if isinstance(m, torch.nn.Dropout)]
+            if len(set(drops)) > 1:
+                raise UnsupportedModel("the dropouts of a block must share p")
+            wb["p"] = drops[0] if drops else 0.0
+            for t, bn in wb["pairs"]:
+                self._check_bn(bn)
+            if wb["residual"]:
+                self._check_bn(blk.residual[1])
+            if wb["separable"] and wb["cout"] % 8:
+                raise UnsupportedModel("pointwise widths must be multiples of 8")
+        for p in model.parameters():
+            if p.dtype != torch.float32:
+                raise UnsupportedModel("training needs fp32 master weights (the model was converted to another dtype)")
+            self.params.append(p)
+        self._index = {id(p): i for i, p in enumerate(self.params)}
+        self.stride = self.walked[0]["stride"]
+        self.features = self.head.in_channels
+
+    @staticmethod
+    def _check_bn(bn):
+        if not (bn.affine and bn.track_running_stats and bn.momentum is not None):
+            raise UnsupportedModel("training needs affine BatchNorm1d with running statistics and a momentum")
+
+    # ------------------------------------------------------------------------------------------------
+    def forward(self, x, seed):
+        """x [N, L] (or [N, 1, L]) -> (log-probs fp32 [N, T, 5], saved state for `backward`)."""
+        if x.dim() == 3:
+            x = x[:, 0, :]
+        dev = x.device
+        x = x.to(torch.float16).contiguous()
+        N, L = x.shape
+        T = (L - 1) // self.stride + 1
+        M = N * T
+        f16 = torch.float16
+        S = dict(x=x, N=N, T=T, M=M, seed=int(seed), blocks=[], unit=0)
+
+        def empty(rows, c):
+            return torch.empty(rows, c, dtype=f16, device=dev)
+
+        def bn_unit(z, bn, act, p, dst, ldo, lpo, res=None):
+            """stats of z (and of the residual branch's zr), then BatchNorm -> act -> dropout into dst."""
+            C = bn.num_features
+            rec = dict(z=z, bn=bn, act=act, p=p, unit=S["unit"], res=res)
+            S["unit"] += 1
+            for key, (zz, b) in (("", (z, bn)),) + ((("_r", res),) if res is not None else ()):
+                mean = torch.empty(C, dtype=torch.float32, device=dev)
+                invstd = torch.empty_like(mean)
+                native.bn_stats(zz, C, M, C, b.eps, b.momentum, mean, invstd, b.running_mean, b.running_var)
+                b.num_batches_tracked.add_(1)
+                rec["mean" + key], rec["invstd" + key] = mean, invstd
+            rec["mask"] = torch.empty(M, C // 8, dtype=torch.uint8, device=dev) if p > 0 else None
+            native.bn_act_fwd(self._bn_args(rec, S), dst, ldo, lpo)
+            return rec
+
+        def out_buffer(i, C):
+            """(tensor, view at frame 0 of chunk 0, pitch, rows per chunk) of block i's output: a zero-haloed buffer when
+            block i + 1 is a dense k > 1 conv, compact rows otherwise."""
+            if i + 1 < len(self.walked):
+                nb = self.walked[i + 1]
+                if not nb["separable"] and nb["k"] > 1:
+                    p = nb["k"] // 2
+                    buf = torch.zeros(N * (T + 2 * p) * C + nb["k"] * C, dtype=f16, device=dev)
+                    return buf, buf[p * C:], C, T + 2 * p
+            buf = empty(M, C)
+            return buf, buf, C, T
+
+        h = None      # (tensor, pitch) of the current block input
+        for i, wb in enumerate(self.walked):
+            blk, act, p = wb["block"], wb["act"], wb["p"]
+            cout = wb["cout"]
+            out, out_v, ld, lp = out_buffer(i, cout)
+            rec = dict(kind=None, out=(out, out_v, ld, lp))
+            if i == 0:
+                conv, bn = wb["pairs"][0]
+                w16 = conv.conv.weight.detach().to(f16).contiguous()
+                z = empty(M, cout)
+                native.conv_first_ex(x, w16, None, native.ACT_NONE, z, cout, T, 0, stride=self.stride)
+                rec.update(kind="first", w=conv.conv.weight, k=wb["k"], bn=bn_unit(z, bn, act, p, out_v, ld, lp))
+            elif not wb["separable"]:
+                conv, bn = wb["pairs"][0]
+                k, cin = wb["k"], wb["cin"]
+                w = conv.conv.weight.detach()
+                w16 = w.permute(0, 2, 1).reshape(cout, k * cin).to(f16).contiguous()      # [Cout][tap * Cin + cin]
+                z = empty(M, cout)
+                pd = k // 2
+                rows_inner = T + 2 * pd
+                native.gemm(h[0], cin, w16, None, z, cout, N * rows_inner, cout, k * cin, rows_inner=rows_inner, valid_inner=T,
+                            stride_outer=T)
+                rec.update(kind="dense", conv=conv.conv, w16=w16, k=k, cin=cin, x=h[0], bn=bn_unit(z, bn, act, p, out_v, ld, lp))
+            else:
+                reps = []
+                hin, R = h[0], len(wb["pairs"])
+                for r, (tcs, bn) in enumerate(wb["pairs"]):
+                    cdw = tcs.depthwise.in_channels
+                    wd16 = tcs.depthwise.weight.detach().to(f16).contiguous()
+                    wp16 = tcs.pointwise.weight.detach()[:, :, 0].to(f16).contiguous()
+                    d = empty(M, cdw)
+                    native.depthwise_conv(hin, cdw, wd16, d, cdw, N, T)
+                    z = empty(M, cout)
+                    native.gemm(d, cdw, wp16, None, z, cout, M, cout, cdw)
+                    rep = dict(tcs=tcs, h=hin, d=d, wd16=wd16, wp16=wp16, cdw=cdw)
+                    if r == R - 1:
+                        res = None
+                        if wb["residual"]:
+                            rconv, rbn = blk.residual[0].conv, blk.residual[1]
+                            wr16 = rconv.weight.detach()[:, :, 0].to(f16).contiguous()
+                            zr = empty(M, cout)
+                            native.gemm(h[0], wb["cin"], wr16, None, zr, cout, M, cout, wb["cin"])
+                            res = (zr, rbn)
+                            rec.update(rconv=rconv, wr16=wr16, x=h[0])
+                        rep["bn"] = bn_unit(z, bn, act, p, out_v, ld, lp, res=res)
+                    else:
+                        hnext = empty(M, cout)
+                        rep["bn"] = bn_unit(z, bn, act, p, hnext, cout, T)
+                        hin = hnext
+                    reps.append(rep)
+                rec.update(kind="separable", reps=reps, cin=wb["cin"])
+            S["blocks"].append(rec)
+            h = (out, ld)
+        feat = h[0]
+        wh16 = self.head.weight.detach()[:, :, 0].to(f16).contiguous()
+        bh16 = None if self.head.bias is None else self.head.bias.detach().to(f16).contiguous()
+        logp = torch.empty(M, 5, dtype=torch.float32, device=dev)
+        native.ctc_head_train_fwd(feat, M, wh16, bh16, logp)
+        S.update(feat=feat, wh16=wh16, logp=logp)
+        return logp.view(N, T, 5), S
+
+    @staticmethod
+    def _bn_args(rec, S):
+        bn = rec["bn"]
+        res = None
+        if rec["res"] is not None:
+            zr, rbn = rec["res"]
+            res = (zr, zr.shape[1], rec["mean_r"], rec["invstd_r"], rbn.weight.detach(), rbn.bias.detach())
+        return native.bn_act_struct(S["M"], bn.num_features, S["T"], rec["act"], rec["p"], S["seed"], rec["unit"], rec["z"],
+                                    rec["z"].shape[1], rec["mean"], rec["invstd"], bn.weight.detach(), bn.bias.detach(),
+                                    residual=res, mask=rec["mask"])
+
+    # ------------------------------------------------------------------------------------------------
+    def backward(self, S, g):
+        """g = dL/dlogp [N, T, 5] -> gradients of `self.params` (fp32, None for parameters the model does not use)."""
+        N, T, M = S["N"], S["T"], S["M"]
+        dev = g.device
+        f16 = torch.float16
+        grads = [None] * len(self.params)
+
+        def put(param, value):
+            grads[self._index[id(param)]] = value.view(param.shape)
+
+        def zeros32(*shape):
+            return torch.empty(*shape, dtype=torch.float32, device=dev)
+
+        g = g.to(torch.float32).contiguous()
+        F = self.features
+        dfeat = torch.empty(M, F, dtype=f16, device=dev)
+        dwh, dbh = zeros32(5, F), zeros32(5)
+        native.ctc_head_bwd(S["feat"], M, S["wh16"], S["logp"], g.view(M, 5), dwh, dbh, dfeat)
+        put(self.head.weight, dwh)
+        if self.head.bias is not None:
+            put(self.head.bias, dbh)
+
+        dy = (dfeat, F, None, 0)      # gradient at the current block's output: (dy, ldy, dy2, ldy2), compact rows
+
+        def bn_bwd(rec, dy, dz_halo=None):
+            """dz (and dzr) of one BatchNorm unit; BatchNorm parameter gradients stored."""
+            bn, C = rec["bn"], rec["bn"].num_features
+            dgamma, dbeta = zeros32(C), zeros32(C)
+            if dz_halo is None:
+                dz = torch.empty(M, C, dtype=f16, device=dev)
+                dz_v, ldo, lpo = dz, C, T
+            else:
+                dz, dz_v, ldo, lpo = dz_halo
+            kw = {}
+            dzr = None
+            if rec["res"] is not None:
+                rbn = rec["res"][1]
+                dzr = torch.empty(M, C, dtype=f16, device=dev)
+                kw = dict(dgamma_r=zeros32(C), dbeta_r=zeros32(C), dzr=dzr)
+            native.bn_act_bwd(self._bn_args(rec, S), dy[0], dy[1], dgamma, dbeta, dz_v, ldo, lpo, dy2=dy[2], ldy2=dy[3], **kw)
+            put(bn.weight, dgamma)
+            put(bn.bias, dbeta)
+            if dzr is not None:
+                put(rbn.weight, kw["dgamma_r"])
+                put(rbn.bias, kw["dbeta_r"])
+            return dz, dzr
+
+        for i in range(len(self.walked) - 1, -1, -1):
+            rec = S["blocks"][i]
+            wb = self.walked[i]
+            cout = wb["cout"]
+            if rec["kind"] == "first":
+                dz, _ = bn_bwd(rec["bn"], dy)
+                dw = zeros32(*rec["w"].shape)
+                native.conv_first_wgrad(dz, cout, S["x"], self.stride, dw)
+                put(rec["w"], dw)
+            elif rec["kind"] == "dense":
+                k, cin = rec["k"], rec["cin"]
+                pd = k // 2
+                rows_inner = T + 2 * pd
+                if k > 1:
+                    buf = torch.zeros(N * rows_inner * cout + k * cout, dtype=f16, device=dev)
+                    dz_halo = (buf, buf[pd * cout:], cout, rows_inner)
+                    dz, _ = bn_bwd(rec["bn"], dy, dz_halo)
+                    dz_v = dz_halo[1]
+                else:
+                    dz, _ = bn_bwd(rec["bn"], dy)
+                    dz_v = dz
+                dw = zeros32(cout, k * cin)
+                native.wgrad_gemm(dz_v, cout, rec["x"], cin, N * rows_inner, cout, k * cin, dw, rows_inner=rows_inner,
+                                  valid_inner=T, lpz=rows_inner)
+                put(rec["conv"].weight, dw.view(cout, k, cin).permute(0, 2, 1).contiguous())
+                # dX[t] = sum_j dz[t - pd + j] W[:, :, k - 1 - j]: the haloed dz against the taps in reverse order
+                wt = rec["conv"].weight.detach().flip(-1).permute(1, 2, 0).reshape(cin, k * cout).to(f16).contiguous()
+                dx = torch.empty(M, cin, dtype=f16, device=dev)
+                native.gemm(dz, cout, wt, None, dx, cin, N * rows_inner, cin, k * cout, rows_inner=rows_inner, valid_inner=T,
+                            stride_outer=T)
+                dy = (dx, cin, None, 0)
+            else:
+                reps = rec["reps"]
+                dh = None
+                dzr = None
+                for r in range(len(reps) - 1, -1, -1):
+                    rep = reps[r]
+                    dz, dzr_r = bn_bwd(rep["bn"], dy if r == len(reps) - 1 else (dh, cout, None, 0))
+                    if dzr_r is not None:
+                        dzr = dzr_r
+                    cdw = rep["cdw"]
+                    dw = zeros32(cout, cdw)
+                    native.wgrad_gemm(dz, cout, rep["d"], cdw, M, cout, cdw, dw)
+                    put(rep["tcs"].pointwise.weight, dw)
+                    dd = torch.empty(M, cdw, dtype=f16, device=dev)
+                    native.gemm(dz, cout, rep["wp16"].t().contiguous(), None, dd, cdw, M, cdw, cout)
+                    dwd = zeros32(*rep["tcs"].depthwise.weight.shape)
+                    native.depthwise_wgrad(dd, cdw, rep["h"], cdw, N, T, dwd)
+                    put(rep["tcs"].depthwise.weight, dwd)
+                    dh = torch.empty(M, cdw, dtype=f16, device=dev)
+                    native.depthwise_conv(dd, cdw, rep["wd16"].flip(-1).contiguous(), dh, cdw, N, T)
+                cin = rec["cin"]
+                if dzr is not None:
+                    dw = zeros32(cout, cin)
+                    native.wgrad_gemm(dzr, cout, rec["x"], cin, M, cout, cin, dw)
+                    put(rec["rconv"].weight, dw)
+                    dxr = torch.empty(M, cin, dtype=f16, device=dev)
+                    native.gemm(dzr, cout, rec["wr16"].t().contiguous(), None, dxr, cin, M, cin, cout)
+                    dy = (dh, cin, dxr, cin)
+                else:
+                    dy = (dh, cin, None, 0)
+        return grads
+
+
+class CtcTrainFunction(torch.autograd.Function):
+    """Autograd node of `CtcTrainPlan`: forward(plan, seed, x, *plan.params) -> fp32 log-probs [N, T, 5]."""
+
+    @staticmethod
+    def forward(ctx, plan, seed, x, *params):
+        logp, saved = plan.forward(x, seed)
+        ctx.plan, ctx.saved = plan, saved
+        return logp
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        grads = ctx.plan.backward(ctx.saved, g)
+        ctx.saved = None
+        return (None, None, None, *grads)

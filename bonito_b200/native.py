@@ -118,6 +118,26 @@ SIGNATURES = {
     "b200_ctc_beam_workspace_bytes": (c_size_t, [c_int, c_longlong, c_int]),
     "b200_ctc_beam_search": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_float, c_float, c_void_p, c_size_t,
                                      c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_wgrad_gemm_workspace_bytes": (c_size_t, [c_longlong, c_int, c_int]),
+    "b200_wgrad_gemm": (c_int, [c_void_p, c_longlong, c_longlong, c_void_p, c_longlong, c_longlong, c_int, c_int, c_int, c_int,
+                                c_void_p, c_void_p, c_void_p]),
+    "b200_depthwise_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b200_depthwise_wgrad": (c_int, [c_void_p, c_longlong, c_void_p, c_longlong, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                     c_void_p]),
+    "b200_conv_first_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "b200_conv_first_wgrad": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p]),
+    "b200_bn_stats_workspace_bytes": (c_size_t, [c_longlong, c_int]),
+    "b200_bn_stats": (c_int, [c_void_p, c_longlong, c_longlong, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                              c_void_p, c_void_p]),
+    "b200_bn_act_fwd": (c_int, [c_void_p, c_void_p, c_longlong, c_longlong, c_void_p]),
+    "b200_bn_act_bwd_workspace_bytes": (c_size_t, [c_longlong, c_int]),
+    "b200_bn_act_bwd": (c_int, [c_void_p, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p]),
+    "b200_ctc_head_train_fwd": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200_ctc_head_bwd_workspace_bytes": (c_size_t, [c_longlong, c_int]),
+    "b200_ctc_head_bwd": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p]),
     "b200_map_minimizers": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "b200_map_anchors": (c_int, [c_void_p, c_longlong, c_void_p, c_int, c_int, c_void_p, c_longlong, c_void_p, c_void_p,
                                  c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -143,6 +163,14 @@ INFLATE_STATUS = {1: "block type 3", 2: "stored block LEN is not the complement 
                   5: "invalid literal/length or distance code", 6: "distance reaches before the member's first byte",
                   7: "output longer than ISIZE", 8: "output shorter than ISIZE", 9: "DEFLATE data ends before the final block",
                   10: "CRC32 mismatch", 11: "member outside the launch's buffers"}
+
+
+class BnActStruct(ctypes.Structure):
+    """`b200_bn_act` of include/bonito_b200.h."""
+    _fields_ = [("m", c_longlong), ("c", c_int), ("t", c_int), ("act", c_int), ("p", c_float), ("seed", ctypes.c_ulonglong),
+                ("unit", c_int), ("z", c_void_p), ("ldz", c_longlong), ("mean", c_void_p), ("invstd", c_void_p),
+                ("gamma", c_void_p), ("beta", c_void_p), ("zr", c_void_p), ("ldzr", c_longlong), ("mean_r", c_void_p),
+                ("invstd_r", c_void_p), ("gamma_r", c_void_p), ("beta_r", c_void_p), ("mask", c_void_p)]
 
 
 class NativeError(RuntimeError):
@@ -768,6 +796,127 @@ def ctc_beam_search(logp, frame_off, frame_len, beam_width, threshold, qscale, q
                                       _ptr(qstring), _ptr(moves), _stream(stream))
     _check(rc, "b200_ctc_beam_search")
     return sequence, qstring, moves
+
+
+# ---- QuartzNet CTC training (b200_wgrad_gemm ... b200_ctc_head_bwd) ----
+def _f32(t, name):
+    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+        raise NativeError(f"{name}: expected a contiguous CUDA fp32 tensor, got {t.dtype} {t.device}")
+    return t
+
+
+def _workspace(nbytes, device):
+    return torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=device)
+
+
+def wgrad_gemm(dz, ldz, x, ldx, m, cout, k, dw, rows_inner=None, valid_inner=None, lpz=None, stream=None):
+    """dw [cout, k] fp32 = dZ^T X over m GEMM rows with the row map of `gemm` (see b200_wgrad_gemm); `dz` / `x` only supply
+    base pointers."""
+    lib = require()
+    if rows_inner is None:
+        rows_inner = valid_inner = m
+    lpz = valid_inner if lpz is None else lpz
+    with torch.cuda.device(dw.device):
+        ws = _workspace(lib.b200_wgrad_gemm_workspace_bytes(int(m), int(cout), int(k)), dw.device)
+        rc = lib.b200_wgrad_gemm(_ptr(dz), int(ldz), int(lpz), _ptr(x), int(ldx), int(m), int(cout), int(k), int(rows_inner),
+                                 int(valid_inner), _ptr(ws), _ptr(_f32(dw, "dw")), _stream(stream))
+    _check(rc, "b200_wgrad_gemm")
+    return dw
+
+
+def depthwise_wgrad(dy, ldy, x, ldx, n, t, dw, stream=None):
+    """dw [C, 1, K] fp32: the depthwise convolution's weight gradient (see b200_depthwise_wgrad)."""
+    lib = require()
+    c, _, k = dw.shape
+    with torch.cuda.device(dw.device):
+        ws = _workspace(lib.b200_depthwise_wgrad_workspace_bytes(int(n), int(t), c, k), dw.device)
+        rc = lib.b200_depthwise_wgrad(_ptr(dy), int(ldy), _ptr(x), int(ldx), int(n), int(t), c, k, _ptr(ws),
+                                      _ptr(_f32(dw, "dw")), _stream(stream))
+    _check(rc, "b200_depthwise_wgrad")
+    return dw
+
+
+def conv_first_wgrad(dz, ldz, x, stride, dw, stream=None):
+    """dw [C, 1, K] fp32: the first convolution's weight gradient against the signal x [N, L] (see b200_conv_first_wgrad)."""
+    lib = require()
+    n, l = x.shape
+    c, _, k = dw.shape
+    t = (l - 1) // stride + 1
+    with torch.cuda.device(dw.device):
+        ws = _workspace(lib.b200_conv_first_wgrad_workspace_bytes(n, t, c, k), dw.device)
+        rc = lib.b200_conv_first_wgrad(_ptr(dz), int(ldz), _ptr(_f16(x, "x")), n, l, c, k, int(stride), _ptr(ws),
+                                       _ptr(_f32(dw, "dw")), _stream(stream))
+    _check(rc, "b200_conv_first_wgrad")
+    return dw
+
+
+def bn_stats(z, ldz, m, c, eps, momentum, mean, invstd, running_mean=None, running_var=None, stream=None):
+    """Batch statistics of z [m, c] (pitch ldz) into mean / invstd, updating the running statistics (see b200_bn_stats)."""
+    lib = require()
+    with torch.cuda.device(mean.device):
+        ws = _workspace(lib.b200_bn_stats_workspace_bytes(int(m), int(c)), mean.device)
+        rc = lib.b200_bn_stats(_ptr(z), int(ldz), int(m), int(c), float(eps), float(momentum), _ptr(ws), _ptr(_f32(mean, "mean")),
+                               _ptr(_f32(invstd, "invstd")), _ptr(running_mean), _ptr(running_var), _stream(stream))
+    _check(rc, "b200_bn_stats")
+
+
+def bn_act_struct(m, c, t, act, p, seed, unit, z, ldz, mean, invstd, gamma, beta, residual=None, mask=None):
+    """A `b200_bn_act`; `residual` = (zr, ldzr, mean_r, invstd_r, gamma_r, beta_r) or None.  The struct holds raw pointers:
+    the caller keeps the tensors alive."""
+    s = BnActStruct(m=int(m), c=int(c), t=int(t), act=int(act), p=float(p), seed=int(seed) & (2**64 - 1), unit=int(unit),
+                    z=z.data_ptr(), ldz=int(ldz), mean=_f32(mean, "mean").data_ptr(), invstd=_f32(invstd, "invstd").data_ptr(),
+                    gamma=_f32(gamma, "gamma").data_ptr(), beta=_f32(beta, "beta").data_ptr(),
+                    mask=None if mask is None else mask.data_ptr())
+    if residual is not None:
+        zr, ldzr, mr, ir, gr, br = residual
+        s.zr, s.ldzr, s.mean_r, s.invstd_r, s.gamma_r, s.beta_r = (zr.data_ptr(), int(ldzr), _f32(mr, "mean_r").data_ptr(),
+                                                                   _f32(ir, "invstd_r").data_ptr(), _f32(gr, "gamma_r").data_ptr(),
+                                                                   _f32(br, "beta_r").data_ptr())
+    return s
+
+
+def bn_act_fwd(args, out, ldo, lpo, stream=None):
+    """BatchNorm [+ residual BatchNorm] -> activation -> dropout into rows of `out` (see b200_bn_act_fwd)."""
+    lib = require()
+    with torch.cuda.device(out.device):
+        rc = lib.b200_bn_act_fwd(ctypes.byref(args), _ptr(out), int(ldo), int(lpo), _stream(stream))
+    _check(rc, "b200_bn_act_fwd")
+    return out
+
+
+def bn_act_bwd(args, dy, ldy, dgamma, dbeta, dz, ldo, lpo, dy2=None, ldy2=0, dgamma_r=None, dbeta_r=None, dzr=None, stream=None):
+    """Gradient of `bn_act_fwd` (see b200_bn_act_bwd)."""
+    lib = require()
+    for t, name in ((dy, "dy"), (dy2, "dy2")):
+        if t is not None and t.stride(-1) != 1:
+            raise NativeError(f"bn_act_bwd: {name} must have unit stride along its last dimension (rows of pitch ld)")
+    with torch.cuda.device(dz.device):
+        ws = _workspace(lib.b200_bn_act_bwd_workspace_bytes(args.m, args.c), dz.device)
+        rc = lib.b200_bn_act_bwd(ctypes.byref(args), _ptr(dy), int(ldy), _ptr(dy2), int(ldy2), _ptr(ws), _ptr(_f32(dgamma, "dgamma")),
+                                 _ptr(_f32(dbeta, "dbeta")), _ptr(dgamma_r), _ptr(dbeta_r), _ptr(dz), _ptr(dzr), int(ldo), int(lpo),
+                                 _stream(stream))
+    _check(rc, "b200_bn_act_bwd")
+
+
+def ctc_head_train_fwd(x, m, w, bias, logp, stream=None):
+    """logp [m, 5] fp32 = log_softmax(fp16(x w^T + bias)) (see b200_ctc_head_train_fwd)."""
+    lib = require()
+    with torch.cuda.device(logp.device):
+        rc = lib.b200_ctc_head_train_fwd(_ptr(_f16(x, "x")), int(m), w.shape[-1], _ptr(_f16(w, "w")), _ptr(bias),
+                                         _ptr(_f32(logp, "logp")), _stream(stream))
+    _check(rc, "b200_ctc_head_train_fwd")
+    return logp
+
+
+def ctc_head_bwd(x, m, w, logp, g, dw, db, dx, stream=None):
+    """Gradient of `ctc_head_train_fwd` from g = dL/dlogp (see b200_ctc_head_bwd)."""
+    lib = require()
+    f = w.shape[-1]
+    with torch.cuda.device(dx.device):
+        ws = _workspace(lib.b200_ctc_head_bwd_workspace_bytes(int(m), f), dx.device)
+        rc = lib.b200_ctc_head_bwd(_ptr(_f16(x, "x")), int(m), f, _ptr(_f16(w, "w")), _ptr(_f32(logp, "logp")), _ptr(_f32(g, "g")),
+                                   _ptr(ws), _ptr(_f32(dw, "dw")), _ptr(db), _ptr(_f16(dx, "dx")), _stream(stream))
+    _check(rc, "b200_ctc_head_bwd")
 
 
 def lstm_crf_fwd(plan_struct, x, scores, stream=None):

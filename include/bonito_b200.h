@@ -237,6 +237,70 @@ int b200_ctc_head_fwd(const void* x, long long m, int f, const void* w, const vo
                       void* stream);
 
 /*
+ * ---- QuartzNet CTC training (reference: bonito/ctc/model.py in train mode behind `bonito train`; the work splits are
+ *      stated in bonito_b200/csrc/ctc_train.cu).  Activations are channels-last fp16 rows [m = n*t][c]; every reduction
+ *      over the rows runs in fixed slices combined in slice order: no atomics, bitwise reproducible.  inf and NaN pass
+ *      through.  Workspaces come from the *_workspace_bytes() queries for the same sizes. ----
+ *
+ * b200_wgrad_gemm: weight gradient dw [cout][k] fp32 = sum over the GEMM rows r of dz[row(r)][co] * x[r * ldx + kk], with
+ *   the row map of b200_gemm_fwd_ex: (outer, inner) = divmod(r, rows_inner), rows with inner >= valid_inner skipped,
+ *   row(r) = outer * lpz + inner.  m % rows_inner == 0; ldx < k gives overlapping x rows (a dense k > 1 convolution over
+ *   a zero-haloed buffer: rows_inner = t + 2 pad, valid_inner = t, kk = tap * cin + ci).  cout, k, ldz, ldx multiples of
+ *   8, dz and x 16-byte aligned.  Split-K over row slices when the workspace query is nonzero.
+ * b200_depthwise_wgrad: dw [c][k] fp32 = sum_{n, i} dy[(n t + i) ldy + ch] x[(n t + i + j - k/2) ldx + ch], frames outside
+ *   [0, t) of chunk n read as zero; 256 <= c <= 512, c % 8 == 0, odd k <= 123.
+ * b200_conv_first_wgrad: dw [c][k] fp32 of the first convolution (1 -> c, padding k/2, `stride`) against the signal x
+ *   [n][l] fp16: sum_{n, i} dz[(n t + i) ldz + ch] x[n][i stride + j - k/2], t = (l - 1) / stride + 1; c % 8 == 0 <= 512,
+ *   odd k <= 33, stride <= 8.
+ * b200_bn_stats: per-channel mean and biased variance of z [m][c] (pitch ldz): mean, invstd = 1/sqrt(var + eps) fp32 [c];
+ *   running_mean / running_var (fp32, or both NULL) are updated in place as torch.nn.BatchNorm1d does in train mode
+ *   (momentum, unbiased variance).  Per-slice Welford partials merged by Chan's formula in slice order.
+ * b200_bn_act_fwd: out row (i / t) * lpo + i % t (pitch ldo) = dropout(act(BN(z) [+ BN_r(zr)])) in fp16, each step
+ *   rounded to fp16 as the module tree rounds under autocast; BN(z) = gamma (z - mean) invstd + beta.  Dropout (p > 0):
+ *   element (i, ch) is kept when the top 24 bits of splitmix64(seed, unit, i * c + ch) are >= p * 2^24, kept values are
+ *   scaled by 1 / (1 - p), and mask [m][c / 8] receives the keep bits (bit j of byte ch / 8 = channel ch with ch % 8 = j).
+ * b200_bn_act_bwd: from dy (+ dy2, summed first) at the output of b200_bn_act_fwd with the same arguments: dgamma, dbeta
+ *   (and dgamma_r, dbeta_r) fp32 [c], dz (and dzr) fp16 at rows (i / t) * lpo + i % t, pitch ldo.
+ * b200_ctc_head_train_fwd: logp [m][5] fp32 = log_softmax(fp16(x w^T + bias)), x [m][f] fp16, f % 8 == 0 <= 2048.
+ * b200_ctc_head_bwd: from g = dL/dlogp [m][5] fp32 and that logp: dw [5][f], db [5] (may be NULL) fp32, dx [m][f] fp16.
+ */
+typedef struct b200_bn_act {
+    long long m;                 /* rows (a multiple of t) */
+    int c, t, act;               /* channels (multiple of 8), frames per chunk, B200_ACT_NONE / _RELU / _SWISH */
+    float p;                     /* dropout probability in [0, 1) */
+    unsigned long long seed;     /* dropout key */
+    int unit;                    /* dropout stream of this layer */
+    const void* z;               /* pre-BatchNorm fp16 [m][ldz] */
+    long long ldz;
+    const float *mean, *invstd, *gamma, *beta;
+    const void* zr;              /* residual branch (NULL: none) */
+    long long ldzr;
+    const float *mean_r, *invstd_r, *gamma_r, *beta_r;
+    void* mask;                  /* [m][c / 8] keep bits (unused when p == 0) */
+} b200_bn_act;
+size_t b200_wgrad_gemm_workspace_bytes(long long m, int cout, int k);
+int b200_wgrad_gemm(const void* dz, long long ldz, long long lpz, const void* x, long long ldx, long long m, int cout, int k,
+                    int rows_inner, int valid_inner, void* workspace, void* dw, void* stream);
+size_t b200_depthwise_wgrad_workspace_bytes(int n, int t, int c, int k);
+int b200_depthwise_wgrad(const void* dy, long long ldy, const void* x, long long ldx, int n, int t, int c, int k, void* workspace,
+                         void* dw, void* stream);
+size_t b200_conv_first_wgrad_workspace_bytes(int n, int t, int c, int k);
+int b200_conv_first_wgrad(const void* dz, long long ldz, const void* x, int n, int l, int c, int k, int stride, void* workspace,
+                          void* dw, void* stream);
+size_t b200_bn_stats_workspace_bytes(long long m, int c);
+int b200_bn_stats(const void* z, long long ldz, long long m, int c, float eps, float momentum, void* workspace, void* mean,
+                  void* invstd, void* running_mean, void* running_var, void* stream);
+int b200_bn_act_fwd(const b200_bn_act* args, void* out, long long ldo, long long lpo, void* stream);
+size_t b200_bn_act_bwd_workspace_bytes(long long m, int c);
+int b200_bn_act_bwd(const b200_bn_act* args, const void* dy, long long ldy, const void* dy2, long long ldy2, void* workspace,
+                    void* dgamma, void* dbeta, void* dgamma_r, void* dbeta_r, void* dz, void* dzr, long long ldo, long long lpo,
+                    void* stream);
+int b200_ctc_head_train_fwd(const void* x, long long m, int f, const void* w, const void* bias, void* logp, void* stream);
+size_t b200_ctc_head_bwd_workspace_bytes(long long m, int f);
+int b200_ctc_head_bwd(const void* x, long long m, int f, const void* w, const void* logp, const void* g, void* workspace, void* dw,
+                      void* db, void* dx, void* stream);
+
+/*
  * Batched Smith-Waterman local alignment with affine gaps (match +5, mismatch -4, gap open 8, extend 4; the tie rules are
  * in bonito_b200/csrc/align.cu), for n_pairs pairs (query p, reference p) of ASCII A/C/G/T bytes.  `query` / `ref` are
  * packed DEVICE byte buffers; pair p is query[query_off[p] .. + query_len[p]) against ref[ref_off[p] .. + ref_len[p]).
